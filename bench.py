@@ -9,8 +9,11 @@ BASELINE.json configs[1] shape (D_W_15K_V1, batch 5000) is measured in the same 
 `bootea_15k` block of the same JSON line (N = 1 only).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload bootea_100k|bootea_15k]
+                    [--dump-outputs DIR]
 
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  --dump-outputs DIR writes what the last timed step left in the tables (a fixed, seeded
+sample of the entity rows, all relation rows, their Adagrad accumulators) and that step's loss as DIR/<name>.npy, so that
+two builds can be compared output for output: with the same arguments the inputs are identical from run to run.
 """
 import argparse
 import json
@@ -24,6 +27,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
+sys.dont_write_bytecode = True     # the tree may be read-only: nothing is written there
 
 WORKLOADS = {
     # BASELINE.json configs[1]; args from the reference's run/args/bootea_args_15K.json
@@ -34,6 +38,7 @@ WORKLOADS = {
                         balance=0.2, name="BootEA D_W_100K_V1 shape (synthetic), dim=100, batch=20000, 10 eps-truncated negatives"),
 }
 L2_FLUSH_BYTES = 512 << 20
+DUMP_ENTITY_ROWS = 32768          # --dump-outputs: seeded sample of the entity table (all of it would exceed 64 MB at 100K)
 SHAPE_ENTITIES = {"15K": 15000, "100K": 100000}      # entities per KG (openea_b200/synth.py SHAPES)
 
 
@@ -42,11 +47,11 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return json.load(f), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi sampling during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampling during the timed region (the clocks line of the JSON result)."""
 
     def __init__(self, index):
         self.index = index
@@ -134,6 +139,20 @@ def build_workload(wl, rank, device, world=1):
     steps_per_epoch = int(np.ceil(T / cfg["batch"]))
     return dict(cfg=cfg, arr=arr, ent=ent, rel=rel, kg1=kg1, kg2=kg2, tset=tset, trainer=trainer,
                 steps_per_epoch=steps_per_epoch, n_triples=T, n_triples_global=n_triples_global)
+
+
+def dump_outputs(out_dir, W, last_loss):
+    """The tables the timed path updated, as float32 arrays (entity rows: a fixed seeded sample), and its last loss."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    ent, rel = W["ent"], W["rel"]
+    idx = np.sort(np.random.default_rng(0).choice(ent.rows, min(ent.rows, DUMP_ENTITY_ROWS), replace=False))
+    sel = torch.as_tensor(idx, device=ent.weight.device)
+    arrays = {"entity_embeddings_sample": ent.raw()[sel], "entity_adagrad_sample": ent.state1[sel, :ent.dim],
+              "relation_embeddings": rel.raw(), "relation_adagrad": rel.state1[:, :rel.dim]}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.float().cpu().numpy())
+    np.save(os.path.join(out_dir, "loss_last_step.npy"), np.array([last_loss], dtype=np.float64))
 
 
 def decode_dbg(dbg, n, t1, t2, k):
@@ -359,7 +378,7 @@ def probe_pipelined_e2e(args):
             got.append(pipe.collect((i - 1) % 2))
     got.append(pipe.collect(5 % 2))
     rel = max(abs(a - b) / max(1e-12, abs(b)) for a, b in zip(got, want))
-    K = max(8, args.steps)
+    K = args.steps
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     for i in range(K):
@@ -501,11 +520,14 @@ def bench_triples(args, wl, rank, local_rank, world, device, full):
         dist.barrier()
     torch.cuda.synchronize()
     n_push0 = 0 if xchg is None else xchg.epoch
+    loss_before_last = None
     with ClockSampler(local_rank) as clocks:
         t_wall0 = time.perf_counter()
         for i in range(K):
             if not args.no_flush:
                 flush.fill_(float(i))   # L2 flush (not timed: outside the event pairs)
+            if full and args.dump_outputs and i == K - 1:
+                loss_before_last = tr.loss_dev.clone()      # outside the event pair, like the flush
             one_step(n_warm + i, evs[i])
         torch.cuda.synchronize()
         t_wall = time.perf_counter() - t_wall0
@@ -519,6 +541,8 @@ def bench_triples(args, wl, rank, local_rank, world, device, full):
         t = torch.tensor([total_ms], dtype=torch.float64, device=device)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         total_ms = float(t.item())
+    if loss_before_last is not None and rank == 0:
+        dump_outputs(args.dump_outputs, W, float((tr.loss_dev - loss_before_last).item()))
     loss_val = tr.read_loss()
     value = world * n_pos_step * K / (total_ms * 1e-3)
 
@@ -558,7 +582,7 @@ def bench_triples(args, wl, rank, local_rank, world, device, full):
     score_med_ms = float(np.median([e[3].elapsed_time(e[1]) for e in evs2]))
     split_step_ms = float(np.mean([e[0].elapsed_time(e[2]) for e in evs2]))
     roofline = {"bound": "hbm", "kernel": "k_step_sampled_duo", "achieved": achieved, "peak": pk["hbm_gbs"], "unit": "GB/s",
-                "frac": achieved / pk["hbm_gbs"], "traffic": traffic, "peak_kind": pk_kind + " (burst copy)",
+                "frac": achieved / pk["hbm_gbs"], "traffic": traffic, "peak_kind": pk_kind,
                 "algorithmic_bytes_per_launch": score_bytes, "bytes_model": "SURVEY 8(d): 24*d per scored triple",
                 "optimiser_bytes": opt_bytes, "achieved_incl_optimiser": (score_bytes + opt_bytes) / (kern_med_ms * 1e-3) / 1e9,
                 "touched_rows_per_step": n_touched,
@@ -578,9 +602,9 @@ def bench_triples(args, wl, rank, local_rank, world, device, full):
                              "mode": xchg.mode, "bytes_per_exchange": xchg.bytes_per_sync, "exchanges_in_timed_region": n_push,
                              "epoch_steps": epoch_steps, "time_to_global_epoch_ms": epoch_steps * total_ms / K,
                              "status": xchg.status(),
-                             "accuracy_note": "this is the north-star's stale-replica scheme: fast, but measured to lose Hits@1 "
-                                              "(15K shape, 100 epochs: 36.4 on one GPU, 19.7 at N=2, 9.2 at N=8); the exact and "
-                                              "delta-sum modes keep it (DESIGN.md section 6, scripts/bench_multi_modes.py)"}
+                             "accuracy_note": "this is the north-star's stale-replica scheme: fast, but it loses Hits@1 against "
+                                              "one GPU, more so as N grows; the exact and delta-sum modes keep it (DESIGN.md "
+                                              "section 6, scripts/bench_multi_modes.py)"}
     if not full:
         if xchg is not None:
             xchg.close()
@@ -624,7 +648,7 @@ def bench_triples(args, wl, rank, local_rank, world, device, full):
     from openea_b200 import engine as eng
     os.environ["OEA_FED_FUSED"] = "1"       # grouped scorer + row optimiser as one cooperative launch per step
     pipe = eng.FedHostPipeline(tr, 3 * (n_pos_h + n_neg_h) + 64)
-    Kp = max(K, 40)
+    Kp = K
     for rep in range(2):                    # rep 0 = warm-up
         if world > 1:
             dist.barrier()
@@ -698,6 +722,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true", help="skip the bootea_15k block and the CSLS block (profiling runs)")
     ap.add_argument("--no-flush", action="store_true", help="diagnostic only: keep L2 warm between timed steps (the number is NOT a valid bench value)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the tables and loss the last timed step produced as DIR/<name>.npy")
     ap.add_argument("--probe-pipelined-e2e", action="store_true",
                     help="internal: measure the depth-2 pipelined host-index step in this process and print its JSON")
     args = ap.parse_args()
@@ -713,7 +739,7 @@ def main():
                            "global epoch over NVLink peer memory") if world > 1 else "single",
               "l2": "flushed between timed steps (512 MiB write)",
               "l2_e2e": "pipelined e2e steps run back to back (no flush possible); per-step working set = tables + gradients + "
-                        "Adagrad slots (%d MB) + candidate lists, vs 126 MB of L2" % (3 * 4 * cfg["dim"] * 2 * SHAPE_ENTITIES.get(cfg["shape"], 0) // 1000000)}
+                        "Adagrad slots (%d MB) + candidate lists, vs 50 MB of L2" % (3 * 4 * cfg["dim"] * 2 * SHAPE_ENTITIES.get(cfg["shape"], 0) // 1000000)}
 
     if args.no_flush:
         config["l2"] = "NOT flushed (diagnostic run, invalid as a bench value)"

@@ -1,5 +1,5 @@
 /*
- * oea.h — C-ABI of liboea.so, the B200 (sm_100a) engine behind the OpenEA hot path.
+ * oea.h — C-ABI of liboea.so, the H100 (sm_90a) engine behind the OpenEA hot path.
  *
  * The reference (nju-websoft/OpenEA) has NO native / FFI layer: its "operator API" is a set of
  * Python callables that bottom out in TensorFlow-1 session.run() and NumPy.  Each entry point
@@ -381,7 +381,7 @@ int oea_sim_rank(const oea_sim_cfg* cfg, const float* e1, const float* e2,
  * approaches/bootea.py:214-219).  Also the first stage of the large-k neighbour search. */
 int oea_sim_matrix(const oea_sim_cfg* cfg, const float* e1, const float* e2,
                    const float* row_off, const float* col_off, float* out, int64_t ld_out, void* stream);
-/* oea_sim_matrix for the inner-product metric on the tensor cores (oea_sim_tc.cu): 3xTF32 tcgen05.mma with fp32 TMEM
+/* oea_sim_matrix for the inner-product metric on the tensor cores (oea_sim_tc.cu): 3xTF32 wgmma with fp32 register
  * accumulators; values agree with oea_sim_matrix to fp32 round-off (not bit for bit: the summation order differs), which
  * is why it is opt-in (OEA_SIM_TC=1 in openea_b200.finding).  Takes the ROW-major operands (e1_t / e2_t are not read);
  * ld_out % 4 == 0.  OEA_ERR_KIND for other metrics. */

@@ -1,4 +1,4 @@
-"""`openea` — drop-in import name of the reference package, served by the B200 engine.
+"""`openea` — drop-in import name of the reference package, served by the CUDA engine.
 
 Every `openea.<x>` module is the SAME module object as `openea_b200.<x>`, so run/main_from_args.py and user
 code written against nju-websoft/OpenEA import unchanged.

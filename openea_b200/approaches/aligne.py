@@ -1,4 +1,4 @@
-"""AlignE on the B200 engine (approaches/aligne.py): limited loss, ε-truncated negatives, swapping."""
+"""AlignE on the CUDA engine (approaches/aligne.py): limited loss, ε-truncated negatives, swapping."""
 from openea_b200.models.basic_model import BasicModel
 from openea_b200.modules.utils.util import load_session
 

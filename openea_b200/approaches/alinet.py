@@ -1,4 +1,4 @@
-"""AliNet on the B200 engine (approaches/alinet.py of the reference): gated multi-hop neighbourhood aggregation.
+"""AliNet on the CUDA engine (approaches/alinet.py of the reference): gated multi-hop neighbourhood aggregation.
 
 Per layer i (dims layer_dims[i] → layer_dims[i+1]):
     one-hop   BN → X·W → A₁·(XW) + b → tanh                        (GraphConvolution.call, alinet.py:574-590)

@@ -1,4 +1,4 @@
-"""AttrE on the B200 engine (approaches/attre.py of the reference; SURVEY §8f-2): three losses per epoch, each with its
+"""AttrE on the CUDA engine (approaches/attre.py of the reference; SURVEY §8f-2): three losses per epoch, each with its
 own SGD instance —
 
   structure     margin TransE on relation triples                                  K1 sampled step (BasicModel)

@@ -1,4 +1,4 @@
-"""BootEA on the B200 engine (approaches/bootea.py): AlignE + bootstrapping of likely alignments.
+"""BootEA on the CUDA engine (approaches/bootea.py): AlignE + bootstrapping of likely alignments.
 
 Per iteration: `sub_epoch` epochs of fused triple steps → validation → bootstrapping (reference-entity
 cosine similarity on the GPU, threshold ∧ top-k filter, matching, editing) → one pass of the alignment loss

@@ -1,4 +1,4 @@
-"""GCN-Align on the B200 engine (approaches/gcn_align.py of the reference).
+"""GCN-Align on the CUDA engine (approaches/gcn_align.py of the reference).
 
 Two independent 2-layer GCNs trained full-batch with SGD (lr = args.learning_rate, 8 in the shipped config):
   SE (structure): layer 1 is featureless, its "weights" are the entity table W0 [N, se_dim], created by
@@ -65,7 +65,7 @@ class GCNAlignUnit:
 
 
 class GraphedTrainStep:
-    """One unit's full-batch train_step (9 kernels + a few memsets for ~60 µs of device work at the 15K shape) captured
+    """One unit's full-batch train_step (9 kernels + a few memsets, tens of microseconds of device work at the 15K shape) captured
     once as a CUDA graph: an epoch is one graph launch instead of a launch-latency-bound chain.  The four negative-index
     vectors live in static buffers (refreshed in place every 10 epochs); the loss stays on the device."""
 

@@ -1,4 +1,4 @@
-"""IMUSE on the B200 engine (approaches/imuse.py of the reference; SURVEY §8f-2).
+"""IMUSE on the CUDA engine (approaches/imuse.py of the reference; SURVEY §8f-2).
 
 Training is TransE with the margin loss (one uniform negative, SGD) on the K1 kernels plus an align loss
 Σ ‖ê₁ − ê₂‖² over the entity pairs a string matcher found before training (imuse.py:303-306,309-322), which is

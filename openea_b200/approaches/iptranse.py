@@ -1,4 +1,4 @@
-"""IPTransE on the B200 engine (approaches/iptranse.py of the reference; SURVEY §8f-2).
+"""IPTransE on the CUDA engine (approaches/iptranse.py of the reference; SURVEY §8f-2).
 
 Three losses over the shared entity / relation tables, all margin-based with one negative per positive:
 

@@ -1,4 +1,4 @@
-"""JAPE on the B200 engine (approaches/jape.py of the reference; SURVEY §8f-2).
+"""JAPE on the CUDA engine (approaches/jape.py of the reference; SURVEY §8f-2).
 
 Structure embedding: the triple loss Σ s⁺ − neg_alpha·Σ s⁻ with s = ‖ĥ + r̂ − t̂‖² (jape.py:72-82), Adagrad — two
 passes of the fed scorer with the positive loss (scale 1 on the positives, −neg_alpha on the negatives) and one row

@@ -1,4 +1,4 @@
-"""MTransE on the B200 engine (approaches/mtranse.py of the reference): positive-only squared-L2 TransE loss
+"""MTransE on the CUDA engine (approaches/mtranse.py of the reference): positive-only squared-L2 TransE loss
 on relation triples + the orthogonal mapping loss on seed pairs, each with its own Adagrad slots."""
 import math
 import time

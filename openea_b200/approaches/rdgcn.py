@@ -1,4 +1,4 @@
-"""RDGCN on the B200 engine (approaches/rdgcn.py of the reference): relation-aware dual-graph convolution.
+"""RDGCN on the CUDA engine (approaches/rdgcn.py of the reference): relation-aware dual-graph convolution.
 
 Graph (Layer.build, rdgcn.py:317-338), X₀ = trainable entity name embeddings [E, d]:
     dual X₁ = [head_rᵀ·X₀/cnt ‖ tail_rᵀ·X₀/cnt]  (compute_r :258-266; the dense [R×E]·[E×d] products of the reference

@@ -1,4 +1,4 @@
-"""SEA on the B200 engine (approaches/sea.py of the reference; SURVEY §8f-2): TransE with the margin loss (one uniform
+"""SEA on the CUDA engine (approaches/sea.py of the reference; SURVEY §8f-2): TransE with the margin loss (one uniform
 negative, Adam) on the K1 kernels + a cycle-consistent pair of mapping matrices trained on labelled and unlabelled
 entity pairs.
 

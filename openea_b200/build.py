@@ -1,7 +1,7 @@
-"""In-tree build of liboea.so (sm_100a only) and of the CPU oracle.
+"""In-tree build of liboea.so (sm_90a only) and of the CPU oracle.
 
-`python -m openea_b200.build` or `__graft_entry__.build()`.  The .so files are git-ignored but travel
-to the GPU box with the gpurun snapshot.
+`python -m openea_b200.build` or `__graft_entry__.build()`.  The .so files and object caches are build products
+(git-ignored), rebuilt from the sources in the tree.
 """
 import hashlib
 import os
@@ -16,7 +16,7 @@ LIB_DIR = os.path.join(HERE, "_lib")
 LIB_PATH = os.path.join(LIB_DIR, "liboea.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "--compiler-options", "-fPIC",
     "-shared",
@@ -87,7 +87,7 @@ def build_cuda(force=False, verbose=False, defines=(), out=None):
             with open(stamp, "w") as f:
                 f.write(digest)
     if relink:
-        cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", out] + objs
+        cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", out] + objs
         res = subprocess.run(cmd, capture_output=True, text=True)
         if res.returncode != 0:
             sys.stderr.write(res.stdout + res.stderr)

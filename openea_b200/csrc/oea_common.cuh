@@ -1,4 +1,4 @@
-// oea_common.cuh — device helpers shared by the liboea kernels (sm_100a only).
+// oea_common.cuh — device helpers shared by the liboea kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -62,43 +62,12 @@ __host__ __device__ __forceinline__ bool aligned16(const void* p) {
     return (reinterpret_cast<uintptr_t>(p) & 15u) == 0;
 }
 
-// ---- packed fp32x2 arithmetic (sm_100: FFMA2 / FADD2 / FMUL2 — one issue slot for two IEEE fp32 results) ---------
-// Same rounding as the scalar forms (fma.rn / add.rn / mul.rn), so results are bit-identical; the kernels here are
-// issue-slot bound, not flop bound, which is why halving the instruction count of the vector maths pays.
-#ifndef OEA_F32X2
-#define OEA_F32X2 1
-#endif
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-#if OEA_F32X2
-    float2 d;
-    asm("{.reg .b64 ra, rb, rc, rd;\n mov.b64 ra, {%2,%3};\n mov.b64 rb, {%4,%5};\n mov.b64 rc, {%6,%7};\n"
-        " fma.rn.f32x2 rd, ra, rb, rc;\n mov.b64 {%0,%1}, rd;}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-    return d;
-#else
-    return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
-#endif
-}
-__device__ __forceinline__ float2 add2(float2 a, float2 b) {
-#if OEA_F32X2
-    float2 d;
-    asm("{.reg .b64 ra, rb, rd;\n mov.b64 ra, {%2,%3};\n mov.b64 rb, {%4,%5};\n add.rn.f32x2 rd, ra, rb;\n mov.b64 {%0,%1}, rd;}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-    return d;
-#else
-    return make_float2(a.x + b.x, a.y + b.y);
-#endif
-}
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-#if OEA_F32X2
-    float2 d;
-    asm("{.reg .b64 ra, rb, rd;\n mov.b64 ra, {%2,%3};\n mov.b64 rb, {%4,%5};\n mul.rn.f32x2 rd, ra, rb;\n mov.b64 {%0,%1}, rd;}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-    return d;
-#else
-    return make_float2(a.x * b.x, a.y * b.y);
-#endif
-}
+// ---- fp32 pair arithmetic ----------------------------------------------------------------------
+// Two independent IEEE fp32 lanes (fma.rn / add.rn / mul.rn each); Hopper has no packed fp32x2 instructions, so these are
+// two scalar operations.
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 lo2(float4 a) { return make_float2(a.x, a.y); }
 __device__ __forceinline__ float2 hi2(float4 a) { return make_float2(a.z, a.w); }
 __device__ __forceinline__ float4 cat4(float2 lo, float2 hi) { return make_float4(lo.x, lo.y, hi.x, hi.y); }

@@ -1,4 +1,4 @@
-// oea_duo.cuh — the octet row layout of path (i) and the "duo" scorer: one warp scores TWO positives at once.  sm_100a.
+// oea_duo.cuh — the octet row layout of path (i) and the "duo" scorer: one warp scores TWO positives at once.  sm_90a.
 //
 // Octet layout (squared-L2 score, pitch <= 128 floats): 8 lanes hold one embedding row, 4 float4 per lane, so the three
 // reductions of a row are 3 shuffle steps and a warp has 4 rows in flight.
@@ -6,8 +6,8 @@
 // Duo scorer: lanes 0-15 work on positive A, lanes 16-31 on positive B of a pair; each half-warp is two octets.  Per
 // positive the negatives are taken two at a time (k = 10: five full rounds instead of three rounds of four with two
 // idle octets), the sampling chain / phase 1 instructions serve two positives, and two independent dependent-load
-// chains are in flight per warp — the kernel is latency/issue bound (profiles/r02_ncu_step_sampled_oct_*.txt:
-// 0.5-0.74 eligible warps per scheduler), not bandwidth bound.  A step of B positives needs B/2 warp tasks, so the
+// chains are in flight per warp — the kernel is latency/issue bound (dependent gathers per positive over L2-resident
+// tables), not bandwidth bound.  A step of B positives needs B/2 warp tasks, so the
 // 5 000-positive step of the 15K shape fits one resident wave without the 2-tasks-vs-1 tail of the octet kernel.
 // Same maths and — for the sampled source — the same draws as k_score_sampled_oct (modules/base/losses.py:15-73,
 // modules/train/batch.py:36-119, initializers.py:26); requires k <= 16.
@@ -59,7 +59,7 @@ __device__ __forceinline__ float cross_oct_sum(float v) {
 #define OEA_DUO_WARPS 4
 #endif
 #ifndef OEA_DUO_MINB
-#define OEA_DUO_MINB 5      // measured on B200 (profiles/r02_ab_duo.txt): 5 CTAs x 4 warps (<= 96 registers, no spills) beats 6 and 8 at both shapes
+#define OEA_DUO_MINB 5      // 5 CTAs x 4 warps: at most 96 registers per thread, no spills
 #endif
 constexpr int kDuoWarps = OEA_DUO_WARPS;
 constexpr int kDuoThreads = kDuoWarps * OEA_WARP;

@@ -1,4 +1,4 @@
-// oea_match.cu — f-4: stable (Gale–Shapley) alignment on the device over K3's top-`cut` lists.  sm_100a.
+// oea_match.cu — f-4: stable (Gale–Shapley) alignment on the device over K3's top-`cut` lists.  sm_90a.
 //
 // Restates modules/finding/alignment.py:171-224 (galeshapley, called by stable_alignment :87-133 with max_iteration =
 // cut = 100): suitors (KG1 rows) propose to the head of their preference list; a reviewer (KG2 column) holds the suitor

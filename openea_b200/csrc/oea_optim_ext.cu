@@ -1,5 +1,5 @@
 // oea_optim_ext.cu — tf.train.AdadeltaOptimizer (modules/base/optimizers.py:13-15 of the reference) as a dense table
-// update.  sm_100a.
+// update.  sm_90a.
 //
 // TF1 ApplyAdadelta (defaults rho = 0.95, epsilon = 1e-8, both slots start at 0), element-wise and in this order:
 //     accum        = rho·accum + (1 − rho)·g²

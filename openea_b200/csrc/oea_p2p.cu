@@ -1,5 +1,5 @@
 // oea_p2p.cu — path (i) across GPUs: the per-epoch exchange of seed-pair rows (SURVEY §8e, BASELINE.json north_star)
-// as direct peer-memory stores over NVLink instead of a library collective.  sm_100a.
+// as direct peer-memory stores over NVLink instead of a library collective.  sm_90a.
 //
 // The reference has no multi-device code (SURVEY §2a); the exchange mirrors what its single session does implicitly:
 // the seed entities of models/basic_model.py:211-236 are the rows both KGs' triples keep coherent.

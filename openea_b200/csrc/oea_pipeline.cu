@@ -1,7 +1,7 @@
 // oea_pipeline.cu — the fed step with HOST index buffers as a depth-2 pipeline: the host→device copy of step i+1
 // overlaps the kernels of step i, and the host reads step i's loss while step i+1 runs.  Same kernels and the same
 // strictly sequential table updates as oea_triple_step_fed_host (the session.run(feed_dict) boundary of
-// models/basic_model.py:222-232); only the copies and the host wait move off the critical path.  sm_100a.
+// models/basic_model.py:222-232); only the copies and the host wait move off the critical path.  sm_90a.
 //
 // Two slots, each with its own device index buffer, device loss scalar and pinned host loss scalar:
 //   submit(slot):   copy stream   wait computed[slot]  (the slot's previous user has finished reading the buffers)

@@ -1,7 +1,7 @@
 // oea_rowmath.cuh — embedding-row arithmetic shared by the path-(i) kernels (oea_triple.cu, oea_triple_ext.cu):
 // a row of `dim` floats held as VEC float4 per lane of one warp, TF's l2_normalize and its Jacobian, the score and
 // loss functions of modules/base/losses.py, the per-block loss accumulator, and the host-side table checks / grid
-// sizing.  sm_100a.
+// sizing.  sm_90a.
 #pragma once
 #include "oea_common.cuh"
 
@@ -150,7 +150,7 @@ inline int sm_count_cached() {
     static int sms = 0;
     if (sms == 0) {
         int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 148;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 132;
     }
     return sms;
 }
@@ -162,7 +162,7 @@ inline int grid_for(int n_warp_items) {
 }
 
 // Exactly one resident wave for kernel `fn` (grid-stride loops do the rest): a partial last wave would run at a
-// fraction of the machine for a whole block duration (measured: 2.11 waves cost 3 block durations).
+// fraction of the machine for a whole block duration.
 template <typename Fn>
 static int grid_one_wave(Fn fn, int n_warp_items, int warps_per_block = kWarpsPerBlock) {
     static int occ = 0;   // one static per kernel instantiation

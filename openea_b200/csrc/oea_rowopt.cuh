@@ -1,5 +1,5 @@
 // oea_rowopt.cuh — the row optimiser phase shared by the one-launch training steps (oea_triple.cu: the sampled step;
-// oea_triple_grouped.cu: the fed step): TF1 Adagrad / SGD on the rows a scorer flagged, in the octet layout.  sm_100a.
+// oea_triple_grouped.cu: the fed step): TF1 Adagrad / SGD on the rows a scorer flagged, in the octet layout.  sm_90a.
 #pragma once
 #include "oea_rowmath.cuh"
 

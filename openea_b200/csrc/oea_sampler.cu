@@ -1,5 +1,5 @@
 // oea_sampler.cu — the batch producer of modules/train/batch.py:36-45 / :168-184 on the device: index vectors for the
-// fed entry points (oea_triple_score_fed, oea_model_score_fed).  sm_100a.
+// fed entry points (oea_triple_score_fed, oea_model_score_fed).  sm_90a.
 #include "oea_sampler.cuh"
 
 namespace oea {

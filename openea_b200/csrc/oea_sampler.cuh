@@ -1,6 +1,6 @@
 // oea_sampler.cuh — the on-device batch sampler of path (i), shared by the fused step kernels (oea_triple.cu) and the
 // batch producer (oea_sampler.cu): step parameters, the counter RNG, negative sampling of one positive by its warp
-// (modules/train/batch.py:89-119), and the host-side slice arithmetic of batch.py:36-53.  sm_100a.
+// (modules/train/batch.py:89-119), and the host-side slice arithmetic of batch.py:36-53.  sm_90a.
 #pragma once
 #include <stdlib.h>
 #include "oea_rowmath.cuh"

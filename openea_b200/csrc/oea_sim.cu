@@ -1,4 +1,4 @@
-// oea_sim.cu — path (iii): all-pairs similarity, CSLS, per-row top-k, rank-of-gold (K3).  sm_100a.
+// oea_sim.cu — path (iii): all-pairs similarity, CSLS, per-row top-k, rank-of-gold (K3).  sm_90a.
 //
 // Restates (no code shared):
 //   modules/finding/similarity.py:11-83   sim(): inner / cosine / euclidean / manhattan, csls_sim()
@@ -138,23 +138,10 @@ k_sim_tile(SimParams P) {
                 const float4 b1 = *reinterpret_cast<const float4*>(&Bs[buf][kk][64 + tx * 4]);
                 const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
                 const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-                if (METRIC == OEA_METRIC_INNER && OEA_F32X2) {
-                    // packed FFMA2: 32 issue slots per k-step instead of 64; per-(i,j) accumulation order unchanged
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const float2 aa = make_float2(a[i], a[i]);
+                for (int i = 0; i < 8; ++i)
 #pragma unroll
-                        for (int j = 0; j < 8; j += 2) {
-                            const float2 r = fma2(aa, make_float2(b[j], b[j + 1]), make_float2(acc[i][j], acc[i][j + 1]));
-                            acc[i][j] = r.x; acc[i][j + 1] = r.y;
-                        }
-                    }
-                } else {
-#pragma unroll
-                    for (int i = 0; i < 8; ++i)
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) acc[i][j] = sim_accum<METRIC>(a[i], b[j], acc[i][j]);
-                }
+                    for (int j = 0; j < 8; ++j) acc[i][j] = sim_accum<METRIC>(a[i], b[j], acc[i][j]);
             }
         }
 
@@ -305,7 +292,7 @@ k_sim_tile(SimParams P) {
 // Short-contraction store kernel (kdim ≤ 104, i.e. the d = 75 / 100 embeddings of MTransE / BootEA): the A panel of the
 // row block ([kdim][128], ≤ 53 KB) is loaded ONCE and stays in shared memory for every column tile; a B tile arrives as
 // two half-K stages ([KH][128] each), so a tile costs 2 block barriers instead of 7 and every load has half a tile of
-// FFMA2 work (≈ 1.7 µs) to land behind.  Same 8×8 register tile, same ascending-k accumulation as k_sim_tile, hence
+// FFMA work to land behind.  Same 8×8 register tile, same ascending-k accumulation as k_sim_tile, hence
 // bit-identical values.  2 CTAs per SM (2 × (2·KH + 2·KH)·128·4 B ≤ 213 KB).
 // ------------------------------------------------------------------------------------------------
 constexpr int SHORTK_MAX = 104;
@@ -372,22 +359,10 @@ k_sim_store_shortk(SimParams P, int KH) {
                 const float4 b1 = *reinterpret_cast<const float4*>(Bb + kk * TN + 64 + tx * 4);
                 const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
                 const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-                if (METRIC == OEA_METRIC_INNER && OEA_F32X2) {
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const float2 aa = make_float2(a[i], a[i]);
+                for (int i = 0; i < 8; ++i)
 #pragma unroll
-                        for (int j = 0; j < 8; j += 2) {
-                            const float2 r = fma2(aa, make_float2(b[j], b[j + 1]), make_float2(acc[i][j], acc[i][j + 1]));
-                            acc[i][j] = r.x; acc[i][j + 1] = r.y;
-                        }
-                    }
-                } else {
-#pragma unroll
-                    for (int i = 0; i < 8; ++i)
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) acc[i][j] = sim_accum<METRIC>(a[i], b[j], acc[i][j]);
-                }
+                    for (int j = 0; j < 8; ++j) acc[i][j] = sim_accum<METRIC>(a[i], b[j], acc[i][j]);
             }
         }
 
@@ -543,7 +518,7 @@ static int sm_count() {
     static int sms = 0;
     if (sms == 0) {
         int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 148;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 132;
     }
     return sms;
 }
@@ -569,7 +544,7 @@ static int launch_sim(const oea_sim_cfg* c, SimParams& P, int splits, cudaStream
 
 // Column splits per row block: the split count that wastes the least of the last wave.  A CTA's time is
 // proportional to its number of column tiles, so with `slots` resident CTAs the kernel takes
-// ceil(row_blocks·splits / slots) · ceil(col_tiles / splits) tile-times; 1.12 waves were measured to cost 2.
+// ceil(row_blocks·splits / slots) · ceil(col_tiles / splits) tile-times: a partial wave costs a whole one.
 static int pick_splits(int n1, int n2) {
     const int row_blocks = (n1 + TM - 1) / TM, col_tiles = (n2 + TN - 1) / TN;
     const long long slots = 2LL * sm_count();              // 2 CTAs per SM (registers and shared memory both allow 2)

@@ -1,31 +1,35 @@
-// oea_sim_tc.cu — path (iii), K3 on the 5th-generation tensor cores: S = E1·E2ᵀ in 3×TF32 (tcgen05.mma kind::tf32, fp32
-// accumulators in TMEM), stored (optionally as the CSLS matrix 2·S − r_i − c_j) for the streaming CSLS passes.  sm_100a.
+// oea_sim_tc.cu — path (iii), K3 on the Hopper tensor cores: S = E1·E2ᵀ in 3×TF32 (wgmma.mma_async m64n128k8 .tf32, fp32
+// accumulators in registers), stored (optionally as the CSLS matrix 2·S − r_i − c_j) for the streaming CSLS passes.  sm_90a.
 //
 // Reference maths: modules/finding/similarity.py:11-54 (`sim`: np.matmul for inner / normalised cosine) and :57-77 (CSLS).
 // The FP32 FFMA tile kernel of oea_sim.cu is the default and the bit-level reference; this kernel is the opt-in fast path
-// (OEA_SIM_TC=1) for the materialised evaluation.  3×TF32: every operand x is split as x = hi + lo with hi = tf32(x) and
-// lo = tf32(x − hi); a·b ≈ lo_a·hi_b + hi_a·lo_b + hi_a·hi_b accumulated in fp32 — the dropped lo·lo term is 2⁻²² relative,
-// below fp32 rounding, so values agree with the FFMA kernel to fp32 round-off (summation order differs).
+// (OEA_SIM_TC=1) for the materialised evaluation and the dense GEMM-NT of the GNN layers.  3×TF32: every operand x is split
+// as x = hi + lo with hi = tf32(x) and lo = x − hi; a·b ≈ lo_a·hi_b + hi_a·lo_b + hi_a·hi_b accumulated in fp32 — the
+// dropped lo·lo term is 2⁻²² relative, below fp32 rounding, so values agree with the FFMA kernel to fp32 round-off
+// (summation order differs).
 //
-// One CTA (256 threads) per 128 × 256 output tile, persistent over tiles, two CTAs per SM so that one CTA's loads and
-// epilogue overlap the other's MMAs (each owns 256 of the SM's 512 TMEM columns and 96 KB of shared memory):
-//   load      all threads read a 32-wide K chunk of the tile's 128 E1 rows and 256 E2 rows (128-bit global loads, every
-//             32-B sector fully used), split hi / lo in registers and store both into the canonical K-major no-swizzle UMMA
-//             layout (8-row × 16-B core matrices: byte = (r/8)·1024 + (k/4)·128 + (r%8)·16 + (k%4)·4);
-//   mma       one elected thread issues 4 k-steps × 3 tcgen05.mma (M = 128, N = 256, K = 8) from shared-memory descriptors
-//             and commits them to an mbarrier; the chunk's buffers are reused once that barrier has flipped;
-//   epilogue  warp w reads TMEM lanes 32(w%4) … +31, column half w/4 (tcgen05.ld 32x32b.x32: one row, 32 columns per thread), applies the
-//             CSLS offsets and writes 128 contiguous bytes per thread and step.
-// Every mbarrier wait is bounded (the kernel traps instead of hanging the device).
+// One CTA (two warpgroups, 256 threads) per 128 × 128 output tile, persistent over tiles, two CTAs per SM so that one CTA's
+// loads and epilogue overlap the other's MMAs.  Per 16-wide K chunk:
+//   load      every thread reads its share of the chunk's 128 E1 rows and 128 E2 rows (128-bit global loads) one chunk
+//             ahead, while the previous chunk's MMAs run; splits hi / lo in registers and stores both into the K-major,
+//             no-swizzle wgmma layout (8-row × 16-B core matrices: byte = (r/8)·512 + (k/4)·128 + (r%8)·16 + (k%4)·4);
+//             two shared-memory buffers alternate between chunks;
+//   mma       warpgroup g issues 2 k-steps × 3 wgmma (M = 64 rows 64g … 64g+63, N = 128, K = 8) from shared-memory
+//             descriptors and keeps at most one chunk's group in flight (wgmma.wait_group 1) before the buffer it read is
+//             refilled;
+//   epilogue  the m64n128 fragment: thread (warp w, lane l) of warpgroup g holds rows 64g + 16(w%4) + l/4 (+8), columns
+//             8j + 2(l%4) (+1) — a quad of lanes writes 32 contiguous bytes of a row, every sector fully used.
 #include <stdlib.h>
 #include "oea_rowmath.cuh"
 
 namespace oea {
 
-constexpr int TCM = 128, TCN = 256, TCK = 32;             // tile rows of E1, rows of E2, K chunk (fp32 elements)
-constexpr int TC_THREADS = 256;
+constexpr int TCM = 128, TCN = 128, TCK = 16;             // tile rows of E1, rows of E2, K chunk (fp32 elements)
+constexpr int TC_THREADS = 256;                           // two warpgroups: rows 0-63 and 64-127 of the tile
 constexpr int TC_A_BYTES = TCM * TCK * 4, TC_B_BYTES = TCN * TCK * 4;
-constexpr int TC_SMEM_BYTES = 2 * TC_A_BYTES + 2 * TC_B_BYTES + 64;   // A hi/lo, B hi/lo, barrier + TMEM pointer
+constexpr int TC_STAGE_BYTES = 2 * TC_A_BYTES + 2 * TC_B_BYTES;     // A hi/lo, B hi/lo: 32 KB
+constexpr int TC_SMEM_BYTES = 2 * TC_STAGE_BYTES;                    // two stages: 64 KB, two CTAs per SM
+constexpr int TC_GROUP_BYTES = 8 * 16 * (TCK / 4);                   // one 8-row group of core matrices across the chunk
 
 struct TcParams {
     const float* e1; const float* e2;
@@ -38,199 +42,36 @@ struct TcParams {
 #ifndef OEA_HOST_EMU
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__device__ __forceinline__ float tf32_round(float x) {
-    uint32_t u;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
-    return __uint_as_float(u);
+// K-major, no-swizzle shared-memory matrix descriptor of wgmma: start address, leading byte offset (between the two 16-B
+// K halves of one K = 8 step) and stride byte offset (between 8-row groups), all >> 4; base offset 0, layout type 0.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32);
 }
 
-// K-major, SWIZZLE_NONE shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout): start address, leading
-// byte offset (between the two 16-B K halves of one MMA) and stride byte offset (between 8-row groups), all >> 4;
-// version = 1 (Blackwell) at bits 46-47; layout type 0.
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-           (1ull << 46);
-}
-
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+// D[64 × 128] (+)= A[64 × 8] · B[128 × 8]ᵀ in TF32, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n"
-        :: "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    for (uint32_t spin = 0; spin < (1u << 27); ++spin) {
-        uint32_t ok;
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                     : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-        if (ok) return;
-    }
-    __trap();      // the MMAs never completed: fail the launch instead of hanging the device
-}
-
-// hi / lo split of a [ROWS × 32] fp32 chunk into the UMMA layout.  256 threads cover 32 rows × 8 sixteen-byte columns per
-// pass; ALL of a thread's loads are issued before the first conversion (ROWS/32 independent 128-bit loads in flight per
-// thread — the first version issued them one at a time and was bound by L2 latency: 16.9 ms for the 70 000² store).
-template <int ROWS>
-__device__ __forceinline__ void stage_chunk(const float* __restrict__ src_base, int pitch, int n_rows, int row0, int k0, int kdim,
-                                            char* hi, char* lo, int tid) {
-    constexpr int PASSES = ROWS / 32;
-    const int r_in = (tid & 7) + 8 * (tid >> 6);          // quarter-warps write whole 128-B core-matrix row groups
-    const int kc = (tid >> 3) & 7;
-    const int k = k0 + 4 * kc;
-    float4 v[PASSES];
-#pragma unroll
-    for (int p = 0; p < PASSES; ++p) {
-        const int r = 32 * p + r_in;
-        v[p] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (row0 + r < n_rows && k < kdim) v[p] = __ldg(reinterpret_cast<const float4*>(src_base + (size_t)(row0 + r) * pitch + k));
-    }
-#pragma unroll
-    for (int p = 0; p < PASSES; ++p) {
-        const int r = 32 * p + r_in;
-        float4 h, l;
-        h.x = tf32_round(v[p].x); h.y = tf32_round(v[p].y); h.z = tf32_round(v[p].z); h.w = tf32_round(v[p].w);
-        l.x = tf32_round(v[p].x - h.x); l.y = tf32_round(v[p].y - h.y); l.z = tf32_round(v[p].z - h.z); l.w = tf32_round(v[p].w - h.w);
-        const int off = (r >> 3) * 1024 + kc * 128 + (r & 7) * 16;
-        *reinterpret_cast<float4*>(hi + off) = h;
-        *reinterpret_cast<float4*>(lo + off) = l;
-    }
-}
-
-__global__ void __launch_bounds__(TC_THREADS, 2)
-k_sim_store_tc(TcParams P) {
-    extern __shared__ __align__(1024) char smem[];
-    char* a_hi = smem;
-    char* a_lo = smem + TC_A_BYTES;
-    char* b_hi = smem + 2 * TC_A_BYTES;
-    char* b_lo = smem + 2 * TC_A_BYTES + TC_B_BYTES;
-    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 2 * TC_A_BYTES + 2 * TC_B_BYTES);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + 1);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const uint32_t bar_addr = smem_u32(bar);
-
-    if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar_addr));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" :: "r"(smem_u32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-
-    // instruction descriptor (cute::UMMA::InstrDescriptor): D = F32 (1 << 4), A = B = TF32 (2 << 7, 2 << 10), both K-major,
-    // N >> 3 at bit 17, M >> 4 at bit 24
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TCN >> 3) << 17) | ((uint32_t)(TCM >> 4) << 24);
-    const int n_chunks = (P.kdim + TCK - 1) / TCK;
-    const long long n_tiles = (long long)P.tiles_m * P.tiles_n;
-    uint32_t parity = 0;
-
-    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int tm = (int)(tile / P.tiles_n), tn = (int)(tile % P.tiles_n);
-        const int row0 = tm * TCM, col0 = tn * TCN;
-        for (int ch = 0; ch < n_chunks; ++ch) {
-            if (ch > 0) { mbar_wait(bar_addr, parity); parity ^= 1u; }       // the previous chunk's MMAs have read the buffers
-            stage_chunk<TCM>(P.e1, P.pitch1, P.n1, row0, ch * TCK, P.kdim, a_hi, a_lo, tid);
-            stage_chunk<TCN>(P.e2, P.pitch2, P.n2, col0, ch * TCK, P.kdim, b_hi, b_lo, tid);
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy stores → visible to the MMA's async reads
-            __syncthreads();
-            if (tid == 0) {
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t ah = smem_u32(a_hi), al = smem_u32(a_lo), bh = smem_u32(b_hi), bl = smem_u32(b_lo);
-#pragma unroll
-                for (int s = 0; s < TCK / 8; ++s) {                          // one MMA = K of 8 = two 16-B core-matrix columns
-                    const uint32_t o = (uint32_t)s * 256u;
-                    const uint64_t dah = umma_desc(ah + o, 128, 1024), dal = umma_desc(al + o, 128, 1024);
-                    const uint64_t dbh = umma_desc(bh + o, 128, 1024), dbl = umma_desc(bl + o, 128, 1024);
-                    mma_tf32(tmem_base, dal, dbh, idesc, (ch | s) != 0 ? 1u : 0u);   // small terms first
-                    mma_tf32(tmem_base, dah, dbl, idesc, 1u);
-                    mma_tf32(tmem_base, dah, dbh, idesc, 1u);
-                }
-                // tcgen05.commit: arrives on the barrier when every MMA issued so far has completed (implies fence::before_thread_sync)
-                asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(bar_addr) : "memory");
-            }
-        }
-        mbar_wait(bar_addr, parity); parity ^= 1u;
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-
-        // ---- epilogue: TMEM lane = tile row; thread (warp, lane) owns row 32·warp + lane ----
-        const int lane_grp = warp & 3, col_half = warp >> 2;      // a warp may read TMEM lanes 32·(warp % 4) … +31 only
-        const int r = row0 + lane_grp * 32 + lane;
-        const bool use_csls = P.row_off != nullptr;
-        const float roff = (use_csls && r < P.n1) ? __ldg(P.row_off + r) : 0.f;
-        float* orow = P.out + (size_t)r * P.ld_out;
-#pragma unroll 1
-        for (int c0 = col_half * (TCN / 2); c0 < (col_half + 1) * (TCN / 2); c0 += 32) {
-            uint32_t v[32];
-            const uint32_t taddr = tmem_base + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)c0;
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                  "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                  "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                  "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                : "r"(taddr) : "memory");
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            if (r < P.n1) {
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                    const int c = col0 + c0 + 4 * q;
-                    float4 o4 = make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                                            __uint_as_float(v[4 * q + 3]));
-                    if (use_csls) {
-                        const float c0f = c < P.n2 ? __ldg(P.col_off + c) : 0.f, c1f = c + 1 < P.n2 ? __ldg(P.col_off + c + 1) : 0.f;
-                        const float c2f = c + 2 < P.n2 ? __ldg(P.col_off + c + 2) : 0.f, c3f = c + 3 < P.n2 ? __ldg(P.col_off + c + 3) : 0.f;
-                        o4.x = (2.f * o4.x - roff) - c0f; o4.y = (2.f * o4.y - roff) - c1f;
-                        o4.z = (2.f * o4.z - roff) - c2f; o4.w = (2.f * o4.w - roff) - c3f;
-                    }
-                    if (c + 3 < P.ld_out && c < P.n2) {          // ld_out is a multiple of 4: whole float4 inside the row's storage
-                        *reinterpret_cast<float4*>(orow + c) = o4;
-                    } else {
-                        if (c < P.n2) orow[c] = o4.x;
-                        if (c + 1 < P.n2) orow[c + 1] = o4.y;
-                        if (c + 2 < P.n2) orow[c + 2] = o4.z;
-                        if (c + 3 < P.n2) orow[c + 3] = o4.w;
-                    }
-                }
-            }
-        }
-        // every warp has drained its TMEM lanes before the next tile's first MMA overwrites the accumulator
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();
-    }
-
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" :: "r"(tmem_base) : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// v3: the same maths as a warp-specialised, double-buffered pipeline (one CTA of 288 threads per SM):
-//   warps 4-11 producers: global → hi/lo split → shared memory, two 96-KB stages (full / empty mbarriers);
-//   warp 12    MMA issuer: 12 tcgen05.mma per stage, tcgen05.commit releases the stage; two 256-column TMEM accumulators;
-//   warps 0-3  epilogue: TMEM → registers → global, releases the accumulator (tmem_full / tmem_empty mbarriers).
-// Loads of chunk c+1, the MMAs of chunk c and the store of the previous tile overlap inside one SM (v2 — one phase at a time per
-// CTA, two CTAs per SM — kept the tensor pipe 25 % busy, profiles/r02_ncu_sim_store_tc_v2.txt).  The split is done with integer
-// ops (round-to-nearest on the magnitude: hi = (bits + 0x1000) & ~0x1FFF, lo = x − hi exactly; the MMA reads lo's top 11 bits):
-// cvt.rna.tf32 ran on the quarter-rate conversion pipe and was 11 % of v2's stall samples.
-constexpr int V3_PRODUCER_WARPS = 8;
-constexpr int V3_THREADS = 32 * (4 + V3_PRODUCER_WARPS + 1);     // 4 epilogue warps, 8 producer warps, the MMA warp
-constexpr int V3_STAGE_BYTES = 2 * TC_A_BYTES + 2 * TC_B_BYTES;            // 96 KB
-constexpr int V3_EPI_LD = 36;                                            // floats per staged row (32 + 4 pad: conflict-free 128-bit accesses)
-constexpr int V3_EPI_BYTES = 4 * 32 * V3_EPI_LD * 4;                       // one 32 × 32 transpose tile per epilogue warp
-constexpr int V3_SMEM_BYTES = 2 * V3_STAGE_BYTES + 128 + V3_EPI_BYTES;
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}\n" :: "r"(bar) : "memory");
-}
+// round-to-nearest split on the magnitude: hi keeps tf32's 10 mantissa bits, lo = x − hi is exact (the MMA reads lo's
+// top 11 bits).  Integer ops: cvt.rna.tf32 runs on the quarter-rate conversion pipe.
 __device__ __forceinline__ void split_store(float4 v, char* hi, char* lo, int off) {
     float4 h, l;
     h.x = __uint_as_float((__float_as_uint(v.x) + 0x1000u) & 0xFFFFE000u); h.y = __uint_as_float((__float_as_uint(v.y) + 0x1000u) & 0xFFFFE000u);
@@ -239,229 +80,99 @@ __device__ __forceinline__ void split_store(float4 v, char* hi, char* lo, int of
     *reinterpret_cast<float4*>(hi + off) = h;
     *reinterpret_cast<float4*>(lo + off) = l;
 }
-// 256 producer threads cover 32 rows × 8 sixteen-byte columns per pass; all of a thread's loads of an operand are in flight
-// together (with 4 producer warps the stage fill took ~6 000 cycles against 1 600 cycles of MMAs per stage: 28 % tensor-pipe
-// activity, profiles/r02_ncu_sim_store_tc3_4producers.txt — the producers' shared-memory stores were the limiter)
-template <int ROWS>
-__device__ __forceinline__ void stage_chunk_v3(const float* __restrict__ src_base, int pitch, int n_rows, int row0, int k0, int kdim,
-                                               char* hi, char* lo, int ptid) {
-    constexpr int PASSES = ROWS / 32;
-    const int r_in = (ptid & 7) + 8 * (ptid >> 6);
-    const int kc = (ptid >> 3) & 7;
-    const int k = k0 + 4 * kc;
-    float4 v[PASSES];
+
+// One operand's share of a [128 × 16] chunk: thread t covers rows (t % 8) + 8·(t / 32) + 64p and the 16-B column
+// (t / 8) % 4, so the 8 threads of a shared-memory phase write 8 different rows of one core matrix (conflict-free) and a
+// warp's loads use whole 32-B sectors.
+struct ChunkRegs { float4 a[2], b[2]; };
+
+__device__ __forceinline__ void load_chunk(const TcParams& P, int row0, int col0, int k0, int tid, ChunkRegs& c) {
+    const int r_in = (tid & 7) + 8 * (tid >> 5), kc = (tid >> 3) & 3, k = k0 + 4 * kc;
 #pragma unroll
-    for (int p = 0; p < PASSES; ++p) {
-        const int r = 32 * p + r_in;
-        v[p] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (row0 + r < n_rows && k < kdim) v[p] = __ldg(reinterpret_cast<const float4*>(src_base + (size_t)(row0 + r) * pitch + k));
-    }
-#pragma unroll
-    for (int p = 0; p < PASSES; ++p) {
-        const int r = 32 * p + r_in;
-        split_store(v[p], hi, lo, (r >> 3) * 1024 + kc * 128 + (r & 7) * 16);
+    for (int p = 0; p < 2; ++p) {
+        const int r = r_in + 64 * p;
+        c.a[p] = c.b[p] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (k < P.kdim) {                                  // kdim % 4 == 0: a 16-B column is all in or all out
+            if (row0 + r < P.n1) c.a[p] = __ldg(reinterpret_cast<const float4*>(P.e1 + (size_t)(row0 + r) * P.pitch1 + k));
+            if (col0 + r < P.n2) c.b[p] = __ldg(reinterpret_cast<const float4*>(P.e2 + (size_t)(col0 + r) * P.pitch2 + k));
+        }
     }
 }
 
-template <bool COALESCED>
-__global__ void __launch_bounds__(V3_THREADS, 1)
-k_sim_store_tc3(TcParams P) {
-    extern __shared__ __align__(1024) char smem[];
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * V3_STAGE_BYTES);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + 2), tfull0 = smem_u32(bars + 4), tempty0 = smem_u32(bars + 6);
-    if (tid == 0) {
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(full0 + 8 * i, 32 * V3_PRODUCER_WARPS); mbar_init(empty0 + 8 * i, 1);
-            mbar_init(tfull0 + 8 * i, 1); mbar_init(tempty0 + 8 * i, 128);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+__device__ __forceinline__ void store_chunk(const ChunkRegs& c, char* stage, int tid) {
+    const int r_in = (tid & 7) + 8 * (tid >> 5), kc = (tid >> 3) & 3;
+#pragma unroll
+    for (int p = 0; p < 2; ++p) {
+        const int r = r_in + 64 * p;
+        const int off = (r >> 3) * TC_GROUP_BYTES + kc * 128 + (r & 7) * 16;
+        split_store(c.a[p], stage, stage + TC_A_BYTES, off);
+        split_store(c.b[p], stage + 2 * TC_A_BYTES, stage + 2 * TC_A_BYTES + TC_B_BYTES, off);
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" :: "r"(smem_u32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
+}
+
+__global__ void __launch_bounds__(TC_THREADS, 2)
+k_sim_store_tc(TcParams P) {
+    extern __shared__ __align__(128) char smem[];
+    const int tid = threadIdx.x, wg = tid >> 7, warp4 = (tid >> 5) & 3, lane = tid & 31;
     const int n_chunks = (P.kdim + TCK - 1) / TCK;
     const long long n_tiles = (long long)P.tiles_m * P.tiles_n;
+    const bool use_csls = P.row_off != nullptr;
 
-    if (warp >= 4 && warp < 4 + V3_PRODUCER_WARPS) {
-        // ===== producers =====
-        const int ptid = tid - 128;
-        uint32_t stage = 0, phase = 0;
-        for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            const int row0 = (int)(tile / P.tiles_n) * TCM, col0 = (int)(tile % P.tiles_n) * TCN;
-            for (int ch = 0; ch < n_chunks; ++ch) {
-                mbar_wait(empty0 + 8 * stage, phase ^ 1u);                 // the MMAs that read this stage have completed
-                char* st = smem + stage * V3_STAGE_BYTES;
-                stage_chunk_v3<TCM>(P.e1, P.pitch1, P.n1, row0, ch * TCK, P.kdim, st, st + TC_A_BYTES, ptid);
-                stage_chunk_v3<TCN>(P.e2, P.pitch2, P.n2, col0, ch * TCK, P.kdim, st + 2 * TC_A_BYTES, st + 2 * TC_A_BYTES + TC_B_BYTES, ptid);
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                mbar_arrive(full0 + 8 * stage);
-                stage ^= 1u; if (stage == 0u) phase ^= 1u;
-            }
-        }
-    } else if (warp == 4 + V3_PRODUCER_WARPS) {
-        // ===== MMA issuer (lane 0 issues; the whole warp walks the barriers) =====
-        const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TCN >> 3) << 17) | ((uint32_t)(TCM >> 4) << 24);
-        uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-        for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            mbar_wait(tempty0 + 8 * acc, acc_phase ^ 1u);                  // the epilogue has drained this accumulator
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            for (int ch = 0; ch < n_chunks; ++ch) {
-                mbar_wait(full0 + 8 * stage, phase);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (lane == 0) {
-                    const uint32_t sb = smem_u32(smem + stage * V3_STAGE_BYTES);
-                    const uint32_t ah = sb, al = sb + TC_A_BYTES, bh = sb + 2 * TC_A_BYTES, bl = sb + 2 * TC_A_BYTES + TC_B_BYTES;
-                    const uint32_t d = tmem_base + acc * 256u;
+    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const int row0 = (int)(tile / P.tiles_n) * TCM, col0 = (int)(tile % P.tiles_n) * TCN;
+        float d[64];
 #pragma unroll
-                    for (int s = 0; s < TCK / 8; ++s) {
-                        const uint32_t o = (uint32_t)s * 256u;
-                        mma_tf32(d, umma_desc(al + o, 128, 1024), umma_desc(bh + o, 128, 1024), idesc, (ch | s) != 0 ? 1u : 0u);
-                        mma_tf32(d, umma_desc(ah + o, 128, 1024), umma_desc(bl + o, 128, 1024), idesc, 1u);
-                        mma_tf32(d, umma_desc(ah + o, 128, 1024), umma_desc(bh + o, 128, 1024), idesc, 1u);
-                    }
-                    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(empty0 + 8 * stage) : "memory");
-                    if (ch == n_chunks - 1)
-                        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(tfull0 + 8 * acc) : "memory");
-                }
-                __syncwarp();
-                stage ^= 1u; if (stage == 0u) phase ^= 1u;
-            }
-            acc ^= 1u; if (acc == 0u) acc_phase ^= 1u;
-        }
-    } else {
-        if constexpr (!COALESCED) {
-        // ===== epilogue (warps 0-3: TMEM lanes 32·warp … +31), direct row-per-thread stores (OEA_SIM_TC_EPI=direct; 12.2 ms at 70 000²) =====
-        uint32_t acc = 0, acc_phase = 0;
-        const bool use_csls = P.row_off != nullptr;
-        for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            const int row0 = (int)(tile / P.tiles_n) * TCM, col0 = (int)(tile % P.tiles_n) * TCN;
-            mbar_wait(tfull0 + 8 * acc, acc_phase);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const int r = row0 + warp * 32 + lane;
-            const float roff = (use_csls && r < P.n1) ? __ldg(P.row_off + r) : 0.f;
-            float* orow = P.out + (size_t)r * P.ld_out;
-#pragma unroll 1
-            for (int c0 = 0; c0 < TCN; c0 += 32) {
-                uint32_t v[32];
-                const uint32_t taddr = tmem_base + acc * 256u + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0;
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                      "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                      "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                      "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                    : "r"(taddr) : "memory");
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                if (r < P.n1) {
+        for (int i = 0; i < 64; ++i) d[i] = 0.f;
+        ChunkRegs regs;
+        load_chunk(P, row0, col0, 0, tid, regs);
+        for (int ch = 0; ch < n_chunks; ++ch) {
+            char* stage = smem + (ch & 1) * TC_STAGE_BYTES;
+            __syncthreads();                  // both warpgroups have retired the MMAs of chunk ch − 2, which read this stage
+            store_chunk(regs, stage, tid);
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy stores → visible to wgmma
+            __syncthreads();
+            asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+            const uint32_t ah = smem_u32(stage) + wg * (64 / 8) * TC_GROUP_BYTES, al = ah + TC_A_BYTES;
+            const uint32_t bh = smem_u32(stage + 2 * TC_A_BYTES), bl = bh + TC_B_BYTES;
 #pragma unroll
-                    for (int q = 0; q < 8; ++q) {
-                        const int c = col0 + c0 + 4 * q;
-                        float4 o4 = make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                                                __uint_as_float(v[4 * q + 3]));
-                        if (use_csls) {
-                            const float c0f = c < P.n2 ? __ldg(P.col_off + c) : 0.f, c1f = c + 1 < P.n2 ? __ldg(P.col_off + c + 1) : 0.f;
-                            const float c2f = c + 2 < P.n2 ? __ldg(P.col_off + c + 2) : 0.f, c3f = c + 3 < P.n2 ? __ldg(P.col_off + c + 3) : 0.f;
-                            o4.x = (2.f * o4.x - roff) - c0f; o4.y = (2.f * o4.y - roff) - c1f;
-                            o4.z = (2.f * o4.z - roff) - c2f; o4.w = (2.f * o4.w - roff) - c3f;
-                        }
-                        if (c + 3 < P.ld_out && c < P.n2) {
-                            *reinterpret_cast<float4*>(orow + c) = o4;
-                        } else {
-                            if (c < P.n2) orow[c] = o4.x;
-                            if (c + 1 < P.n2) orow[c + 1] = o4.y;
-                            if (c + 2 < P.n2) orow[c + 2] = o4.z;
-                            if (c + 3 < P.n2) orow[c + 3] = o4.w;
-                        }
-                    }
+            for (int s = 0; s < TCK / 8; ++s) {                      // one K = 8 step = two 16-B core-matrix columns
+                const uint32_t o = (uint32_t)s * 256u;
+                wgmma_tf32(d, gmma_desc(al + o, 128, TC_GROUP_BYTES), gmma_desc(bh + o, 128, TC_GROUP_BYTES), (ch | s) != 0 ? 1u : 0u);
+                wgmma_tf32(d, gmma_desc(ah + o, 128, TC_GROUP_BYTES), gmma_desc(bl + o, 128, TC_GROUP_BYTES), 1u);   // small terms first
+                wgmma_tf32(d, gmma_desc(ah + o, 128, TC_GROUP_BYTES), gmma_desc(bh + o, 128, TC_GROUP_BYTES), 1u);
+            }
+            asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+            if (ch + 1 < n_chunks) load_chunk(P, row0, col0, (ch + 1) * TCK, tid, regs);   // in flight behind the MMAs
+            asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+        }
+        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+
+        // ---- epilogue: straight from the accumulator fragment ----
+        const int rbase = row0 + 64 * wg + 16 * warp4 + (lane >> 2);
+        float roff[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int r = rbase + 8 * h;
+            roff[h] = (use_csls && r < P.n1) ? __ldg(P.row_off + r) : 0.f;
+        }
+#pragma unroll
+        for (int j = 0; j < TCN / 8; ++j) {
+            const int c = col0 + 8 * j + 2 * (lane & 3);
+            const float c0f = (use_csls && c < P.n2) ? __ldg(P.col_off + c) : 0.f;
+            const float c1f = (use_csls && c + 1 < P.n2) ? __ldg(P.col_off + c + 1) : 0.f;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = rbase + 8 * h;
+                float2 o2 = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+                if (use_csls) { o2.x = (2.f * o2.x - roff[h]) - c0f; o2.y = (2.f * o2.y - roff[h]) - c1f; }
+                if (r < P.n1 && c < P.n2) {
+                    float* orow = P.out + (size_t)r * P.ld_out;
+                    if (c + 1 < P.ld_out) *reinterpret_cast<float2*>(orow + c) = o2;   // ld_out % 4 == 0, c even: 8-B aligned
+                    else orow[c] = o2.x;
                 }
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(tempty0 + 8 * acc);
-            acc ^= 1u; if (acc == 0u) acc_phase ^= 1u;
-        }
-        } else {
-        // ===== epilogue, shared-memory transposed (default; 11.1 ms at 70 000², profiles/r02_sim_tc_v3c_70000.json) =====
-        // tcgen05.ld hands a thread one ROW's 32 columns; written out directly, a warp store instruction would touch 32 rows
-        // × 16 B (32 half-filled sectors — the 70 000² store ran at 1.6 TB/s that way).  Each warp transposes its 32 × 32 block
-        // through a padded shared-memory tile so that a store instruction covers 4 rows × 128 contiguous bytes.
-        float* tile = reinterpret_cast<float*>(smem + 2 * V3_STAGE_BYTES + 128) + warp * 32 * V3_EPI_LD;
-        uint32_t acc = 0, acc_phase = 0;
-        const bool use_csls = P.row_off != nullptr;
-        const int sub_r = lane >> 3, sub_c = (lane & 7) * 4;            // store mapping: rows sub_r + 4j, columns sub_c … +3
-        for (long long tile_i = blockIdx.x; tile_i < n_tiles; tile_i += gridDim.x) {
-            const int row0 = (int)(tile_i / P.tiles_n) * TCM + warp * 32, col0 = (int)(tile_i % P.tiles_n) * TCN;
-            mbar_wait(tfull0 + 8 * acc, acc_phase);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            float roff[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const int r = row0 + sub_r + 4 * j;
-                roff[j] = (use_csls && r < P.n1) ? __ldg(P.row_off + r) : 0.f;
-            }
-#pragma unroll 1
-            for (int c0 = 0; c0 < TCN; c0 += 32) {
-                uint32_t v[32];
-                const uint32_t taddr = tmem_base + acc * 256u + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0;
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                      "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                      "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                      "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                    : "r"(taddr) : "memory");
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                __syncwarp();                                   // the previous step's reads of the tile are done
-#pragma unroll
-                for (int q = 0; q < 8; ++q)
-                    *reinterpret_cast<uint4*>(tile + lane * V3_EPI_LD + 4 * q) = make_uint4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-                __syncwarp();
-                const int c = col0 + c0 + sub_c;
-                float4 coff = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (use_csls) {
-                    coff.x = c < P.n2 ? __ldg(P.col_off + c) : 0.f; coff.y = c + 1 < P.n2 ? __ldg(P.col_off + c + 1) : 0.f;
-                    coff.z = c + 2 < P.n2 ? __ldg(P.col_off + c + 2) : 0.f; coff.w = c + 3 < P.n2 ? __ldg(P.col_off + c + 3) : 0.f;
-                }
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const int rl = sub_r + 4 * j, r = row0 + rl;
-                    float4 o4 = *reinterpret_cast<const float4*>(tile + rl * V3_EPI_LD + sub_c);
-                    if (use_csls) {
-                        o4.x = (2.f * o4.x - roff[j]) - coff.x; o4.y = (2.f * o4.y - roff[j]) - coff.y;
-                        o4.z = (2.f * o4.z - roff[j]) - coff.z; o4.w = (2.f * o4.w - roff[j]) - coff.w;
-                    }
-                    if (r < P.n1) {
-                        float* orow = P.out + (size_t)r * P.ld_out;
-                        if (c + 3 < P.ld_out && c < P.n2) {
-                            *reinterpret_cast<float4*>(orow + c) = o4;
-                        } else {
-                            if (c < P.n2) orow[c] = o4.x;
-                            if (c + 1 < P.n2) orow[c + 1] = o4.y;
-                            if (c + 2 < P.n2) orow[c + 2] = o4.z;
-                            if (c + 3 < P.n2) orow[c + 3] = o4.w;
-                        }
-                    }
-                }
-            }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(tempty0 + 8 * acc);
-            acc ^= 1u; if (acc == 0u) acc_phase ^= 1u;
-        }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" :: "r"(tmem_base) : "memory");
 }
 #endif  // OEA_HOST_EMU
 
@@ -486,23 +197,12 @@ extern "C" int oea_sim_matrix_tc(const oea_sim_cfg* c, const float* e1, const fl
     static bool attr_set = false;
     if (!attr_set) {
         OEA_CUDA_TRY(cudaFuncSetAttribute(k_sim_store_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
-        OEA_CUDA_TRY(cudaFuncSetAttribute(k_sim_store_tc3<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, V3_SMEM_BYTES));
-        OEA_CUDA_TRY(cudaFuncSetAttribute(k_sim_store_tc3<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, V3_SMEM_BYTES));
         attr_set = true;
     }
     const long long tiles = (long long)P.tiles_m * P.tiles_n;
-    const char* v2 = getenv("OEA_SIM_TC_V2");            // A/B: the one-phase-at-a-time kernel (two CTAs per SM)
-    if (v2 != nullptr && v2[0] == '1') {
-        const long long cap = 2ll * sm_count_cached();
-        const int grid = (int)(tiles < cap ? tiles : cap);
-        k_sim_store_tc<<<grid, TC_THREADS, TC_SMEM_BYTES, (cudaStream_t)stream>>>(P);
-    } else {
-        const long long cap = sm_count_cached();
-        const int grid = (int)(tiles < cap ? tiles : cap);
-        const char* epi = getenv("OEA_SIM_TC_EPI");      // "direct": row-per-thread stores (A/B); default = the transposed epilogue
-        if (epi != nullptr && epi[0] == 'd') k_sim_store_tc3<false><<<grid, V3_THREADS, V3_SMEM_BYTES, (cudaStream_t)stream>>>(P);
-        else k_sim_store_tc3<true><<<grid, V3_THREADS, V3_SMEM_BYTES, (cudaStream_t)stream>>>(P);
-    }
+    const long long cap = 2ll * sm_count_cached();
+    const int grid = (int)(tiles < cap ? tiles : cap);
+    k_sim_store_tc<<<grid, TC_THREADS, TC_SMEM_BYTES, (cudaStream_t)stream>>>(P);
     OEA_LAUNCH_CHECK();
     return OEA_OK;
 #else

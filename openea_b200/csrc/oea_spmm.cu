@@ -1,5 +1,5 @@
 // oea_spmm.cu — path (ii): sparse-adjacency × dense-embedding neighbour aggregation (K2) and the
-// L1 margin alignment loss of the GNN approaches.  sm_100a.
+// L1 margin alignment loss of the GNN approaches.  sm_90a.
 //
 // Restates (no code shared):
 //   approaches/gcn_align.py:79-86,239-267   dot(sparse) = tf.sparse_tensor_dense_matmul ; GraphConvolution
@@ -224,7 +224,7 @@ static int spmm_sm_count() {
     static int sms = 0;
     if (sms == 0) {
         int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 148;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 132;
     }
     return sms;
 }

@@ -1,5 +1,5 @@
 // oea_triple.cu — path (i): negative-sampled triple scoring forward+backward (K1), the row
-// optimiser, the fused on-device sampler, and the table lookup.  sm_100a.
+// optimiser, the fused on-device sampler, and the table lookup.  sm_90a.
 //
 // Maths restated from the reference (no code shared):
 //   modules/base/losses.py:15-73      score + losses (sums, squared L2)
@@ -287,7 +287,7 @@ k_score_sampled(TableDev ent, TableDev rel, SampledParams P, oea_loss_cfg cfg,
 #define OEA_OCT_WARPS 4
 #endif
 #ifndef OEA_OCT_MINB
-#define OEA_OCT_MINB 6       // measured on B200 (scripts/ab_score.sh): 6 CTAs × 4 warps, ≤ 80 registers beats both 5 and 8
+#define OEA_OCT_MINB 6       // 6 CTAs × 4 warps: at most 80 registers per thread
 #endif
 #ifndef OEA_OCT_E_SMEM
 #define OEA_OCT_E_SMEM 1
@@ -518,7 +518,7 @@ k_score_sampled_oct(TableDev ent, TableDev rel, const __grid_constant__ SampledP
 }
 
 // The whole sampled training step as ONE cooperative launch: score + gradients, grid barrier, row optimiser.
-// Saves the second launch and its ramp (≈ 6 µs of a 43 µs step at the 15K shape); the grid is one resident wave by
+// Saves the second launch and its ramp; the grid is one resident wave by
 // construction (grid_one_wave), which is what a cooperative launch requires.
 template <int KIND>
 __global__ void __launch_bounds__(kOctThreads, OEA_OCT_MINB)

@@ -1,5 +1,5 @@
 // oea_triple_ext.cu — path (i), SURVEY §8f-2: the other score functions of the reference's models/ on the
-// fed boundary (index vectors in, gradients scattered into the tables), one warp per triple.  sm_100a.
+// fed boundary (index vectors in, gradients scattered into the tables), one warp per triple.  sm_90a.
 //
 // Maths restated from the reference (no code shared):
 //   models/trans/transh.py:25-51        TransH   e⊥ = e − <e, n̂> n̂,  n̂ = l2_normalize(normal_vector[r])

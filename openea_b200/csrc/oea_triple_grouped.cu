@@ -5,7 +5,7 @@
 // them loads one row, and the gradients of the shared rows are summed in registers (the Jacobian of l2_normalize is
 // linear in the incoming gradient) and leave as three vector reductions per positive instead of three per triple:
 // 3 + k row loads and 3 + k row reductions per positive instead of 3·(1 + k) each.  A negative that shares fewer than
-// two rows with its positive (any fed batch is legal) takes the general path of k_score_fed for that triple.  sm_100a.
+// two rows with its positive (any fed batch is legal) takes the general path of k_score_fed for that triple.  sm_90a.
 //
 // Opt-in: oea_triple_step_fed_host uses it when OEA_FED_GROUPED=1 (until it has been timed on hardware);
 // tests/test_emu_triple_grouped.py checks it on the CPU warp emulator against the C oracle.

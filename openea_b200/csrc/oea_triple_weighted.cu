@@ -12,7 +12,7 @@
 //
 // Same row arithmetic, normalisation Jacobian and loss accumulation as oea_triple.cu (oea_rowmath.cuh); one warp per
 // pair, the six (two) rows of a pair in registers.  HBM / L2 bound: 6·4·d B gathered per pair, up to as much reduced.
-// sm_100a.
+// sm_90a.
 #include "oea_rowmath.cuh"
 
 using namespace oea;

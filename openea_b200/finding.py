@@ -61,7 +61,7 @@ def kmajor(t, tc=None):
 
 def _cfg(metric, e1, e2, d, tc=None):
     if metric not in _METRICS:
-        raise ValueError("metric %r is not supported by the B200 engine (inner/cosine/euclidean/manhattan)" % (metric,))
+        raise ValueError("metric %r is not supported by the CUDA engine (inner/cosine/euclidean/manhattan)" % (metric,))
     assert e1.is_contiguous() and e2.is_contiguous()
     t1, ld1 = kmajor(e1, tc)
     t2, ld2 = kmajor(e2, tc) if e2 is not e1 else (t1, ld1)
@@ -145,9 +145,9 @@ MATERIALIZE_MAX_BYTES = 48 << 30   # CSLS runs on a stored n1×n2 matrix (1 cont
 
 
 def use_tensor_cores(metric):
-    """OEA_SIM_TC=1 routes the stored similarity matrix of the materialised evaluation through the 3xTF32 tcgen05 kernel
+    """OEA_SIM_TC=1 routes the stored similarity matrix of the materialised evaluation through the 3xTF32 wgmma kernel
     (oea_sim_matrix_tc; inner / normalised-cosine only).  Off by default: its values equal the FP32 kernel's only to fp32
-    round-off, so arg-max / rank may differ on exact near-ties (measured: profiles/r02_sim_tc_agreement.json)."""
+    round-off, so arg-max / rank may differ on exact near-ties (tests/test_sim_tc_gpu.py bounds how many)."""
     import os
     return os.environ.get("OEA_SIM_TC") == "1" and _METRICS[metric] == L.METRIC_INNER
 

@@ -105,7 +105,7 @@ class SpmmFn(torch.autograd.Function):
 
 
 def tc_gemm_nt(A, B):
-    """C = A·Bᵀ for row-major fp32 A [m, k], B [n, k] (k % 4 == 0) on the tensor cores: the 3xTF32 tcgen05 kernel of path
+    """C = A·Bᵀ for row-major fp32 A [m, k], B [n, k] (k % 4 == 0) on the tensor cores: the 3xTF32 wgmma kernel of path
     (iii) (oea_sim_matrix_tc) used as a GEMM-NT; values agree with an FP32 GEMM to fp32 round-off.  Returns [m, n]."""
     lib = L.load()
     m, k = A.shape

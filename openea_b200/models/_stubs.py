@@ -1,4 +1,4 @@
-"""Importable placeholders for reference classes that are OUT OF SCOPE of the B200 hot path (SURVEY §2:
+"""Importable placeholders for reference classes that are OUT OF SCOPE of the CUDA hot path (SURVEY §2:
 attribute/literal encoders, RNN paths, graph matching, FFT/conv/complex KGE models).  They keep
 run/main_from_args.py importable; using one fails loudly instead of silently running something else."""
 from openea_b200.models.basic_model import BasicModel

@@ -1,5 +1,5 @@
 """BasicModel: the 6-call lifecycle set_args / set_kgs / init / run / test / save of the reference
-(models/basic_model.py) over the B200 engine.
+(models/basic_model.py) over the CUDA engine.
 
 What changed underneath (the lifecycle, printed lines and files on disk are the reference's):
   * variables are device tables (openea_b200.engine.EmbeddingTable), the "graph" is a TripleTrainer;
@@ -122,10 +122,10 @@ class BasicModel:
     # ---- one process per GPU (SURVEY §8e-i) ----------------------------------------------------------------------
     def _multi_mode(self):
         """How path (i) trains under torchrun (DESIGN.md §6).  'exact' (default): replicated tables, every step's batch
-        sharded over the ranks, gradients all-reduced, identical updates — the accuracy of one GPU (Hits@1 36.4 = 36.4 at
-        N = 2 and N = 8), no speed-up at these table sizes.  'seed': the north-star's stale-replica scheme that bench.py
-        times (head-owner triple shards, seed-pair rows exchanged once per epoch over NVLink) — fast, but it loses accuracy
-        (Hits@1 36.4 → 19.7 at N = 2, 9.2 at N = 8 on the 15K shape), so it is opt-in: args.multi_gpu_mode or OEA_MULTI_MODE."""
+        sharded over the ranks, gradients all-reduced, identical updates — the accuracy of one GPU, no speed-up at these
+        table sizes.  'seed': the north-star's stale-replica scheme that bench.py
+        times (head-owner triple shards, seed-pair rows exchanged once per epoch over NVLink) — fast, but it loses accuracy,
+        more as N grows, so it is opt-in: args.multi_gpu_mode or OEA_MULTI_MODE."""
         mode = getattr(self.args, "multi_gpu_mode", None) or os.environ.get("OEA_MULTI_MODE") or "exact"
         if mode not in ("exact", "seed"):
             raise ValueError("multi_gpu_mode must be 'exact' or 'seed', not %r" % (mode,))

@@ -18,7 +18,7 @@ four KG objects before the first training step, while a training epoch on the GP
 Anything this path does not cover exactly (unordered ids — they depend on Python set iteration order —, RSN4EA's
 `remove_unlinked`, the DBP15K / DWY100K layouts, attribute lines that need the reference's multi-tab value joining)
 falls back to the container-based loader in kgs.py, which mirrors the reference line by line.
-tests/test_host_modules.py compares both loaders with the live reference in all three id modes.
+tests/test_host_modules.py compares both loaders with the reference's recorded results in all three id modes.
 """
 import csv
 import hashlib

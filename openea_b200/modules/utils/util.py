@@ -10,7 +10,7 @@ class EngineSession:
         import torch
         from openea_b200 import lib
         if not torch.cuda.is_available():
-            raise lib.OeaError("the B200 engine needs a CUDA device; there is no CPU fallback")
+            raise lib.OeaError("the CUDA engine needs a CUDA device; there is no CPU fallback")
         lib.load()
         self.device = torch.device("cuda", torch.cuda.current_device())
 

@@ -9,7 +9,7 @@
         negative links, backward, gradient sync, TF-Adam — the reference's one step per epoch at 100K.  The one-hop adjacency
         is the symmetric 0/1 matrix of the synthetic D_*_100K-shape triples; the two-hop matrix is a random sparse pattern with
         the real dataset's order of nnz (SURVEY Appendix B: 1.4-2.6·10⁶) because the Zipf hubs of the synthetic graph make its
-        true two-hop neighbourhood 60× denser than D_Y_100K's (profiles/r01_alinet_graph_build_cpu.json).
+        true two-hop neighbourhood far denser than D_Y_100K's.
  rdgcn  (config 5): the RDGCN layer (approaches/rdgcn.py:162-338, d = 300) row-sharded (parallel_gnn.ShardedRDGCNLayer) on the
         100K V2-shape graph (600 000 triples per KG), one training step, plus the 100 000 × 100 000 CSLS evaluation
         (manhattan... the reference's eval metric is inner on d = 300 here) row-sharded over the same ranks.

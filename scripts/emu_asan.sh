@@ -4,7 +4,7 @@
 set -e
 cd "$(dirname "$0")/.."
 OUT=${OEA_EMU_ASAN_LIB:-/tmp/libemu_oea_asan.so}
-g++ -std=c++20 -O0 -pthread -fPIC -shared -DOEA_HOST_EMU -DOEA_F32X2=0 -fsanitize=address -fno-omit-frame-pointer \
+g++ -std=c++20 -O0 -pthread -fPIC -shared -DOEA_HOST_EMU -fsanitize=address -fno-omit-frame-pointer \
     -Wno-attributes -Wno-unknown-pragmas -I "${CUDA_HOME:-/usr/local/cuda}/include" -o "$OUT" tests/emu/emu_kernels.cpp \
     -L"${CUDA_HOME:-/usr/local/cuda}/lib64" -lcudart
 OEA_EMU_LIB="$OUT" LD_PRELOAD="$(gcc -print-file-name=libasan.so)" ASAN_OPTIONS=detect_leaks=0:halt_on_error=1 \

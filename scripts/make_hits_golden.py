@@ -31,8 +31,7 @@ def one_seed(job):
     # The reference trains its FIRST epoch on the triple lists in load order (they are shuffled only after every epoch,
     # models/basic_model.py:234-235) — on the real datasets that is Python-set order, i.e. effectively random, but
     # synth_id_arrays emits np.unique-SORTED triples: an epoch of batches with contiguous head ids inflates Adagrad's
-    # accumulators early and leaves the run ~6 epochs behind for good (measured: Hits@1 34.8 vs 36.4 at epoch 100,
-    # profiles/r02_hits_parity_15k.md).  The oracle therefore starts from a seeded random order, as real data would.
+    # accumulators early and leaves the run several epochs behind for good.  The oracle therefore starts from a seeded random order, as real data would.
     prng = np.random.default_rng(1000 + seed)
     arr["triples1"] = arr["triples1"][prng.permutation(len(arr["triples1"]))]
     arr["triples2"] = arr["triples2"][prng.permutation(len(arr["triples2"]))]

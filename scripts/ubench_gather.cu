@@ -1,4 +1,4 @@
-// Micro-benchmarks that bound the triple scorer (K1) at the 15K / 100K shapes on sm_100a — the questions left open by
+// Micro-benchmarks that bound the triple scorer (K1) at the 15K / 100K shapes on sm_90a — the questions left open by
 // DESIGN.md §4 "where the scorer's time goes":
 //   1. rows/s of independent 400-B row gathers (4 lanes × 16 B … one warp per row, 128-bit loads) from a table that is
 //      L2-resident (12 MB) or not (320 MB), as a function of the rows each warp has in flight (1, 2, 4, 8);
@@ -8,7 +8,7 @@
 //   4. cost of one cooperative grid barrier at one CTA per SM and at full occupancy;
 //   5. the same independent gathers as 1-D bulk async copies (cp.async.bulk = TMA's linear mode, one elected lane per
 //      row, completion on an mbarrier) into shared memory — does TMA staging beat 25 lanes × ld.global.v4 for 400-B rows?
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -rdc=false -o scripts/ubench_gather.bin scripts/ubench_gather.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -rdc=false -o scripts/ubench_gather.bin scripts/ubench_gather.cu
 // Run on the GPU box: scripts/ubench_gather.bin > gpurun_out/ubench_gather.txt
 #include <cooperative_groups.h>
 #include <cstdio>

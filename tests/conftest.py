@@ -13,7 +13,7 @@ os.environ.setdefault("OEA_CACHE_DIR", os.path.join(tempfile.gettempdir(), "oea_
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device, an H100 (select with -m gpu)")
     config.addinivalue_line("markers", "first_hw_run: exercises code that has not yet executed on a GPU; collected last, strict "
                                        "(OEA_QUARANTINE=1 opts into xfail reporting)")
 

@@ -26,7 +26,7 @@ def build(force=False):
         return None
     if not force and os.path.exists(OUT) and all(os.path.getmtime(OUT) >= os.path.getmtime(d) for d in DEPS):
         return OUT
-    cmd = ["g++", "-std=c++20", "-O1", "-pthread", "-fPIC", "-shared", "-DOEA_HOST_EMU", "-DOEA_F32X2=0",
+    cmd = ["g++", "-std=c++20", "-O1", "-pthread", "-fPIC", "-shared", "-DOEA_HOST_EMU",
            "-Wno-attributes", "-Wno-unknown-pragmas", "-I", inc, "-o", OUT, SRC,
            "-L", os.path.join(os.path.dirname(inc), "lib64"), "-lcudart"]
     res = subprocess.run(cmd, capture_output=True, text=True)

@@ -296,6 +296,8 @@ inline float __uint_as_float(unsigned u) { float f; memcpy(&f, &u, 4); return f;
 inline int __float_as_int(float f) { int i; memcpy(&i, &f, 4); return i; }
 inline float __int_as_float(int i) { float f; memcpy(&f, &i, 4); return f; }
 inline unsigned __umulhi(unsigned a, unsigned b) { return (unsigned)(((uint64_t)a * (uint64_t)b) >> 32); }
+inline float __fadd_rn(float a, float b) { return a + b; }
+inline float __fmul_rn(float a, float b) { return a * b; }
 inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }
 inline float emu_expf(float x) { return expf(x); }
 #define __expf emu_expf

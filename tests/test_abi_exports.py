@@ -25,9 +25,11 @@ def test_load_and_error_strings_without_gpu():
     assert rc == 1
 
 
-def test_sm100a_only():
-    """The shared object carries sm_100a SASS (no multi-arch fatbin)."""
+def test_sm90a_only():
+    """The shared object carries sm_90a SASS (no multi-arch fatbin)."""
     import subprocess
-    out = subprocess.run(["cuobjdump", "-lelf", L.LIB_PATH], capture_output=True, text=True).stdout
+    from openea_b200 import build
+    cuobjdump = os.path.join(os.path.dirname(build._nvcc()), "cuobjdump")     # the toolkit's bin need not be on PATH
+    out = subprocess.run([cuobjdump, "-lelf", L.LIB_PATH], capture_output=True, text=True).stdout
     archs = {line.split(".")[-2] for line in out.splitlines() if ".cubin" in line}
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs

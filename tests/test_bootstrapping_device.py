@@ -166,8 +166,6 @@ def test_bootea_device_iteration_methods_on_cpu_tensors(monkeypatch):
     assert ents1b.numel() >= ents1.numel()
 
 
-@pytest.mark.skipif(__import__("oracle.reference_source", fromlist=["x"]).bootea_helpers() is None,
-                    reason="/root/reference not present on this box")
 def test_host_and_device_functions_equal_the_reference_source():
     """The label-editing, swap-triple and batch-slicing functions of BootEA, executed from the reference's own source
     (approaches/bootea.py:35-137), against this package's host functions and the tensor versions."""
@@ -177,7 +175,8 @@ def test_host_and_device_functions_equal_the_reference_source():
     from openea_b200.approaches import bootea as host
     from openea_b200.modules.bootstrapping import device as dev
     from oracle import reference_source
-    ref = reference_source.bootea_helpers()
+    from tests.helpers import ReferenceRecording
+    ref = ReferenceRecording("reference_bootea", reference_source.bootea_helpers)
     rng = np.random.default_rng(3)
     n = 40
     for trial in range(5):
@@ -187,8 +186,8 @@ def test_host_and_device_functions_equal_the_reference_source():
         pre = {(int(i), int(j)) for i, j in zip(rng.permutation(n)[:15], rng.integers(0, n, 15))}
         cur = {(int(i), int(j)) for i, j in zip(rng.permutation(n)[:20], rng.permutation(n)[:20])}     # a matching
         with contextlib.redirect_stdout(io.StringIO()):
-            want_x = ref["update_labeled_alignment_x"](set(pre), set(cur), sim)
-            want_y = ref["update_labeled_alignment_y"](set(want_x), sim)
+            want_x = ref("update_labeled_alignment_x", set(pre), set(cur), sim)
+            want_y = ref("update_labeled_alignment_y", set(want_x), sim)
             assert host.update_labeled_alignment_x(set(pre), set(cur), pair_sim) == want_x
             assert host.update_labeled_alignment_y(set(want_x), pair_sim) == want_y
     # swap triples: dict walk of the reference vs host mirror vs masked gathers on tensors
@@ -206,7 +205,7 @@ def test_host_and_device_functions_equal_the_reference_source():
     e1 = [int(x) for x in rng.permutation(30)[:12]]
     e2 = [int(x) for x in 30 + rng.permutation(30)[:12]]
     with contextlib.redirect_stdout(io.StringIO()):
-        w1, w2 = ref["generate_supervised_triples"](rt1, hr1, rt2, hr2, e1, e2)
+        w1, w2 = ref("generate_supervised_triples", rt1, hr1, rt2, hr2, e1, e2)
         g1, g2 = host.generate_supervised_triples(rt1, hr1, rt2, hr2, e1, e2)
     assert sorted(g1) == sorted(w1) and sorted(g2) == sorted(w2)
     t1 = dev.swap_triples(torch.as_tensor(tri.astype(np.int32)), torch.as_tensor(e1), torch.as_tensor(e2), 60)
@@ -215,7 +214,8 @@ def test_host_and_device_functions_equal_the_reference_source():
     # batch slices
     a, b = [tuple(x) for x in tri.tolist()], [tuple(x) for x in tri2.tolist()]
     for step in range(0, 9):
-        want = ref["generate_pos_batch"](a, b, step, 64)
+        want = ref("generate_pos_batch", a, b, step, 64)
         assert host.generate_pos_batch(a, b, step, 64) == want
         got = dev.pos_batch(torch.as_tensor(tri.astype(np.int32)), torch.as_tensor(tri2.astype(np.int32)), step, 64)
         assert [tuple(x) for x in got.t().tolist()] == list(want[0]) + list(want[1])
+    ref.save()

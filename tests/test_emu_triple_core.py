@@ -1,7 +1,7 @@
 """CPU: the core of path (i) — oea_triple.cu's fed scorers, the row optimisers, the normalised lookup and its backward,
 the tensor-level losses, the on-device triple set and the warp-per-positive sampled scorer — executed from the product's
 kernel SOURCE on the warp emulator (tests/emu) through the product's own Python engine over CPU tensors, against the C
-oracle.  These kernels are verified on the B200 by tests/test_triple_gpu.py; here the same checks guard refactors where
+oracle.  These kernels are verified on the GPU by tests/test_triple_gpu.py; here the same checks guard refactors where
 no GPU exists.  The octet scorer and the one-launch step (a cooperative kernel, run as one block here) are at the end."""
 import ctypes as C
 

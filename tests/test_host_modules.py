@@ -1,6 +1,6 @@
 """CPU tests of the host-side mirror of the reference interface: args, task_divide, batch slicing, id
-assignment, dataset loading (against goldens generated from the reference and, where present, the live
-reference), the host sampler's rules, Gale-Shapley, early_stop, and the `openea` drop-in import surface."""
+assignment, dataset loading (against goldens generated from the reference and the reference's recorded
+results), the host sampler's rules, Gale-Shapley, early_stop, and the `openea` drop-in import surface."""
 import ast
 import contextlib
 import io
@@ -165,16 +165,15 @@ def _reference_kgs(folder, modes):
         sys.modules.update(saved)
 
 
-@pytest.mark.skipif(not ref_adapter.available(), reason="/root/reference not present on this box")
 @pytest.mark.parametrize("loader", ["arrays", "containers", "arrays-cached"])
 def test_dataset_loading_equals_live_reference(tmp_path, monkeypatch, loader):
-    """Full read_kgs_from_folder equivalence with the live reference on a synthetic folder, in all three id modes, for
+    """Full read_kgs_from_folder equivalence with the reference (its recorded results) on a synthetic folder, in all three id modes, for
     the array-backed loader (fresh parse and binary cache) and the container-based loader: id dicts, triple sets and
     lists incl. swap triples, every derived dict, vocabularies, counts, links, URI-level KGs."""
     from openea_b200.modules.load import fast
     from openea_b200.modules.load.kgs import read_kgs_from_folder
     from openea_b200.synth import write_dataset
-    folder = str(tmp_path) + "/"
+    folder = str(tmp_path) + "/data/"        # the binary cache stays outside the dataset folder
     write_dataset(folder, "tiny")
     monkeypatch.setenv("OEA_CACHE_DIR", str(tmp_path) + "/cache")
     if loader == "containers":
@@ -187,7 +186,10 @@ def test_dataset_loading_equals_live_reference(tmp_path, monkeypatch, loader):
     if loader == "arrays-cached":
         assert log.getvalue().count("loaded from cache") == 3
     assert isinstance(mine["mapping"], fast.ArrayKGs) == (loader != "containers")
-    theirs = _reference_kgs(folder, modes)
+    from tests.helpers import ReferenceRecording
+    ref = ReferenceRecording("reference_kgs_synthetic", lambda: {"read_kgs": _reference_kgs})
+    theirs = ref("read_kgs", folder, modes)
+    ref.save()
     for m in mine:
         a, b = mine[m], theirs[m]
         assert a.entities_num == b.entities_num and a.relations_num == b.relations_num and a.attributes_num == b.attributes_num
@@ -218,7 +220,6 @@ def test_dataset_loading_equals_live_reference(tmp_path, monkeypatch, loader):
         assert set(a.useful_entities_list1) == set(b.useful_entities_list1)
 
 
-@pytest.mark.skipif(not ref_adapter.available(), reason="/root/reference not present on this box")
 @pytest.mark.parametrize("case", ["clean", "dirty"])
 def test_array_loader_edge_cases_equal_live_reference(tmp_path, monkeypatch, case):
     """Hand-written folder: duplicate lines, padded fields, values with a trailing '.', an entity that only carries
@@ -245,7 +246,10 @@ def test_array_loader_edge_cases_equal_live_reference(tmp_path, monkeypatch, cas
         mine = {m: read_kgs_from_folder(folder, "721_5fold/1/", m, True) for m in modes}
     assert isinstance(mine["mapping"], fast.ArrayKGs) == (case == "clean")
     assert ("array-backed loader not applicable" in log.getvalue()) == (case == "dirty")
-    theirs = _reference_kgs(folder, modes)
+    from tests.helpers import ReferenceRecording
+    ref = ReferenceRecording("reference_kgs_edge_%s" % case, lambda: {"read_kgs": _reference_kgs})
+    theirs = ref("read_kgs", folder, modes)
+    ref.save()
     for m in modes:
         a, b = mine[m], theirs[m]
         assert (a.entities_num, a.relations_num, a.attributes_num) == (b.entities_num, b.relations_num, b.attributes_num)
@@ -369,20 +373,19 @@ def test_pair_set_behaves_like_the_reference_set():
 
 
 def test_galeshapley_port_equals_the_reference_function():
-    """The host restatement of galeshapley against the reference's own function (imported live with TF stubbed) on
-    random preference structures, including max_iteration cut-offs that stop before everybody is matched."""
-    from oracle import ref_adapter
-    if not ref_adapter.available():
-        pytest.skip("reference sources not present")
+    """The host restatement of galeshapley against the reference's own function (its recorded results) on random
+    preference structures, including max_iteration cut-offs that stop before everybody is matched."""
     import copy
     from openea_b200.modules.finding.alignment import arg_sort, galeshapley
-    ref = ref_adapter.load().alignment
+    from tests.helpers import ReferenceRecording
+    ref = ReferenceRecording("reference_galeshapley", lambda: {"galeshapley": ref_adapter.load().alignment.galeshapley})
     rng = np.random.default_rng(5)
     for n1, n2, cut in ((12, 12, 100), (20, 15, 100), (15, 20, 3), (30, 30, 2)):
         s = rng.standard_normal((n1, n2)).astype(np.float32)
         a = arg_sort(list(range(n1)), s, "x_", "y_"); b = arg_sort(list(range(n2)), s.T, "y_", "x_")
         if n1 > n2 and cut >= n2:
             continue      # more suitors than reviewers and unlimited rounds: the reference runs lists empty (IndexError)
-        want = ref.galeshapley(copy.deepcopy(a), copy.deepcopy(b), cut)
+        want = ref("galeshapley", copy.deepcopy(a), copy.deepcopy(b), cut)
         got = galeshapley(copy.deepcopy(a), copy.deepcopy(b), cut)
         assert got == want, (n1, n2, cut)
+    ref.save()

@@ -1,4 +1,4 @@
-"""GPU: the tensor-core similarity kernel (oea_sim_matrix_tc: 3xTF32 tcgen05.mma, TMEM accumulators) against the FP32 FFMA
+"""GPU: the tensor-core similarity kernel (oea_sim_matrix_tc: 3xTF32 wgmma, register accumulators) against the FP32 FFMA
 kernel (oea_sim_matrix) — values to fp32 round-off on ragged shapes, every K-chunk count, with and without the CSLS offsets;
 and the materialised CSLS evaluation with OEA_SIM_TC=1 against the default path (modules/finding/similarity.py:11-77)."""
 import numpy as np
@@ -8,13 +8,14 @@ import torch
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("n1,n2,d", [(128, 256, 32), (1000, 777, 100), (300, 1300, 75), (513, 511, 300), (257, 300, 8), (64, 40, 36), (2000, 3000, 100)])
+# 128 x 128 output tiles, 16-wide K chunks: shapes on, just past and just short of each boundary, one and many chunks,
+# a grid of more tiles than resident CTAs (persistent loop), and a single row / column
+@pytest.mark.parametrize("n1,n2,d", [(128, 256, 32), (1000, 777, 100), (300, 1300, 75), (513, 511, 300), (257, 300, 8), (64, 40, 36),
+                                     (2000, 3000, 100), (1, 1, 4), (129, 127, 16), (127, 129, 20), (256, 128, 12), (100, 5, 128),
+                                     (5, 100, 132), (40000, 300, 64)])
 @pytest.mark.parametrize("csls", [False, True])
-@pytest.mark.parametrize("variant", ["v3", "v2"])
-def test_tc_matrix_equals_fp32_matrix(cuda_device, monkeypatch, n1, n2, d, csls, variant):
-    """v3 = warp-specialised double-buffered pipeline (default); v2 = one phase at a time per CTA (OEA_SIM_TC_V2=1)."""
+def test_tc_matrix_equals_fp32_matrix(cuda_device, n1, n2, d, csls):
     from openea_b200 import finding as F
-    monkeypatch.setenv("OEA_SIM_TC_V2", "1" if variant == "v2" else "0")
     rng = np.random.default_rng(n1 + d)
     e1, _ = F.to_device_rows(rng.standard_normal((n1, d)).astype(np.float32), False)
     e2, _ = F.to_device_rows(rng.standard_normal((n2, d)).astype(np.float32), False)

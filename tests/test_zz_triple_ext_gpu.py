@@ -101,8 +101,7 @@ def test_transe_through_the_model_entry_equals_the_k1_kernel(cuda_device):
     tb.score_fed(_dev(pos), _dev(neg))
     assert ta.read_loss() == pytest.approx(tb.read_loss(), rel=1e-6)
     for x, y in zip(a[:2], b[:2]):
-        # two kernels, two summation orders: agreement to fp32 rounding of the row reductions (first B200 run: 1 of
-        # 200 000 coordinates differed by 2.5e-5 relative)
+        # two kernels, two summation orders: agreement to fp32 rounding of the row reductions
         np.testing.assert_allclose(x.grad.cpu().numpy(), y.grad.cpu().numpy(), rtol=1e-4, atol=1e-6)
         assert torch.equal(x.touched, y.touched)
 
@@ -298,7 +297,7 @@ def test_score_family_lifecycle(cuda_device, tiny_kgs, tmp_path, name):
     assert len(loss) == 120
     if name == "DistMult":
         # reduce_mean over the batch + Adagrad at lr 0.01 on unit rows (distmult.py:58-59): the loss sits at
-        # steps·ln 2 and moves in the 4th digit over 120 epochs (B200: 3.4661 → 3.4658); it must not grow
+        # steps·ln 2 and moves only in the 4th digit over 120 epochs; it must not grow
         assert abs(loss[0] - 5 * np.log(2.0)) < 0.01 and loss[-1] <= loss[0] * 1.001, (loss[0], loss[-1])
     else:
         assert loss[-1] < 0.9 * loss[0], (loss[0], loss[-1])
@@ -322,7 +321,7 @@ def test_bootea_transh_lifecycle(cuda_device, tiny_kgs, tmp_path):
     assert "avg. triple loss" in out and "generating neighbors of" in out and "Training ends. Total time" in out
     loss = _losses(out, "avg. triple loss:")
     assert loss[-1] < loss[0]
-    assert _hits1(out, "accurate results:") > 4.0        # chance = 0.24 %; BootEA (TransE) reaches > 8 % at 300 epochs
+    assert _hits1(out, "accurate results:") > 4.0        # chance = 0.24 %
 
 
 def test_resume_from_checkpoint_continues_the_same_run(cuda_device, tiny_kgs, tmp_path):
