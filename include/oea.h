@@ -242,22 +242,36 @@ int oea_triple_step_fed_host(const oea_table* ent, const oea_table* rel,
  *   TRANSD    the same on e⊥ = l2_normalize(e + <e, e_p>·r_p)      models/trans/transd.py:26-65
  *   DISTMULT  similarity Σ ĥ∘r̂∘t̂                                  models/semantic/distmult.py:43-59
  *   SIMPLE    (Σ l2n(h_H∘r₁)∘t_T + Σ l2n(t_H∘r₂)∘h_T)/2            models/semantic/simple.py:50-86
- * The two similarity models are scored as energies E = −similarity, so OEA_LOSS_LOGISTIC gives their
- * softplus(−score⁺) + softplus(score⁻). */
-enum { OEA_MODEL_TRANSE = 0, OEA_MODEL_TRANSH = 1, OEA_MODEL_TRANSD = 2, OEA_MODEL_DISTMULT = 3, OEA_MODEL_SIMPLE = 4 };
+ *   ROTATE    Σ_i |ĥ_i·e^{iθ_i} − t̂_i| − γ over (re, im) pairs,      models/semantic/rotate.py:52-110,
+ *             θ = r̂·phase                                          approaches/bootea_rotate.py:48-108,149-160
+ *   HOLE      similarity σ(<l2n(r̂), ccorr(ĥ, t̂)>), ccorr_k = Σ_i ĥ_i·t̂_{(i+k) mod dim}   models/semantic/hole.py:41-86
+ * The similarity models are scored as energies E = −similarity, so OEA_LOSS_LOGISTIC gives their
+ * softplus(−score⁺) + softplus(score⁻).  ROTATE's energy is the distance minus γ, so OEA_LOSS_LOGISTIC is the reference's
+ * −log σ(γ − d⁺) − log σ(d⁻ − γ) and OEA_LOSS_LOGSIGMOID its alignment loss −log σ(γ − d).
+ * ROTATE and HOLE run in fp32 like every other kind (the reference keeps RotatE's variables in float64); the gradient of
+ * RotatE's modulus at a zero coordinate is 0 (TF's is NaN there).  HOLE computes the correlation directly, O(dim²). */
+enum { OEA_MODEL_TRANSE = 0, OEA_MODEL_TRANSH = 1, OEA_MODEL_TRANSD = 2, OEA_MODEL_DISTMULT = 3, OEA_MODEL_SIMPLE = 4,
+       OEA_MODEL_ROTATE = 5, OEA_MODEL_HOLE = 6 };
 
 typedef struct oea_model {
     int32_t kind;              /* OEA_MODEL_* */
-    const oea_table* ent;      /* ent_embeds                                 | SIMPLE: head_ent_embeds */
+    const oea_table* ent;      /* ent_embeds                                 | SIMPLE: head_ent_embeds | ROTATE: re_ent_embeds */
     const oea_table* rel;      /* rel_embeds                                 | SIMPLE: rel_embeds1 */
-    const oea_table* ent_aux;  /* TRANSD: ent_transfer                       | SIMPLE: tail_ent_embeds | else NULL */
+    const oea_table* ent_aux;  /* TRANSD: ent_transfer | SIMPLE: tail_ent_embeds | ROTATE: im_ent_embeds | else NULL */
     const oea_table* rel_aux;  /* TRANSH: normal_vector, TRANSD: rel_transfer | SIMPLE: rel_embeds2   | else NULL */
+    float gamma;               /* ROTATE: γ (args.gamma); ignored by the other kinds */
+    float phase;               /* ROTATE: π/ρ with ρ = (γ + 2)/dim, the scale from r̂ to the phase (rotate.py:37,90);
+                                * ignored by the other kinds */
 } oea_model;
 
 /* oea_triple_score_fed for any oea_model: gathers the 3–6 rows of every triple, scores it, evaluates the loss of
  * modules/base/losses.py and scatter-adds d(loss)/d(raw variable) into the grad of every table involved (setting
  * `touched`).  MARGIN pairs positive i with negative i (n_pos == n_neg).  loss_scale multiplies loss and gradient
  * (1 for TF's reduce_sum losses; 1/(n_pos+n_neg) for DistMult's reduce_mean, distmult.py:58).
+ * ROTATE takes every loss but MARGIN (OEA_ERR_KIND); a negative weight other than the positives' (1/k in rotate.py:81)
+ * is a second call with only negatives.  HOLE takes only MARGIN (OEA_ERR_KIND otherwise), with n_neg = k·n_pos
+ * negatives in the reference layout (those of positive p at p·k … p·k+k−1): Σ_p relu(m + E⁺_p − mean_j E⁻_{p,j})
+ * (hole.py:80-84); OEA_ERR_SHAPE when n_pos does not divide n_neg.
  * All tables share dim and pitch, pitch <= 256.  Run oea_rowopt_apply on every table afterwards. */
 int oea_model_score_fed(const oea_model* model,
                         const int32_t* pos_h, const int32_t* pos_r, const int32_t* pos_t, int32_t n_pos,

@@ -1,6 +1,7 @@
 from openea_b200.approaches.aligne import AlignE
 from openea_b200.approaches.attre import AttrE
 from openea_b200.approaches.bootea import BootEA
+from openea_b200.approaches.bootea_rotate import BootEA_RotatE
 from openea_b200.approaches.bootea_transh import BootEA_TransH
 from openea_b200.approaches.imuse import IMUSE
 from openea_b200.approaches.iptranse import IPTransE
@@ -17,4 +18,3 @@ RSN4EA = out_of_scope("RSN4EA", "recurrent skipping network over paths")
 MultiKE = out_of_scope("MultiKE", "multi-view literal/attribute encoders")
 GMNN = out_of_scope("GMNN", "graph matching network")
 KDCoE = out_of_scope("KDCoE", "description encoder co-training")
-BootEA_RotatE = out_of_scope("BootEA_RotatE", "float64 complex rotation score")

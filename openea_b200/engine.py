@@ -376,18 +376,27 @@ class TripleTrainer:
 
 
 MODEL_KINDS = {"TransE": L.MODEL_TRANSE, "TransH": L.MODEL_TRANSH, "TransD": L.MODEL_TRANSD,
-               "DistMult": L.MODEL_DISTMULT, "SimplE": L.MODEL_SIMPLE}
+               "DistMult": L.MODEL_DISTMULT, "SimplE": L.MODEL_SIMPLE, "RotatE": L.MODEL_ROTATE, "HolE": L.MODEL_HOLE}
+
+ROTATE_EPSILON = 2.0      # rotate.py:25: the embedding range is (γ + ε) / dim
+
+
+def rotate_phase(gamma, dim):
+    """π/ρ with ρ = (γ + 2)/dim: the factor that turns a relation entry into its phase (rotate.py:37,86,90)."""
+    return math.pi / ((float(gamma) + ROTATE_EPSILON) / int(dim))
 
 
 class ModelTrainer:
     """Forward/backward + optimiser for the score functions beyond plain translation (oea_model_score_fed):
-    TransH / TransD / DistMult / SimplE graphs of the reference's models/ (SURVEY §8f-2).
+    TransH / TransD / DistMult / SimplE / RotatE / HolE graphs of the reference's models/ (SURVEY §8f-2).
 
     tables = (ent, rel, ent_aux, rel_aux) EmbeddingTables in the slot order of `oea_model` (None where a model has
     no such table).  A step = device batch producer (oea_triple_sample_batch) → fed scorer → one row-optimiser
-    launch per table; `mean_loss` applies DistMult's reduce_mean (distmult.py:58)."""
+    launch per table; `mean_loss` applies DistMult's reduce_mean (distmult.py:58).  `gamma`: RotatE's γ (the phase
+    scale follows from it and the dimension).  `neg_weight`: weight of the negatives' loss relative to the positives'
+    (RotatE's 1/k, rotate.py:81); None = the same weight."""
 
-    def __init__(self, model, tables, loss, lr, mean_loss=False, sampler="fast"):
+    def __init__(self, model, tables, loss, lr, mean_loss=False, sampler="fast", gamma=None, neg_weight=None):
         self.lib = L.load()
         self.kind = MODEL_KINDS[model]
         self.tables = tuple(tables) + (None,) * (4 - len(tables))
@@ -395,6 +404,11 @@ class ModelTrainer:
         self.loss, self.lr = loss, float(lr)
         self.mean_loss = bool(mean_loss)
         self.sampler = {"fast": 0, "independent": 1}[sampler]
+        if self.kind == L.MODEL_ROTATE and gamma is None:
+            raise ValueError("RotatE needs its margin gamma")
+        self.gamma = 0.0 if gamma is None else float(gamma)
+        self.phase = rotate_phase(gamma, self.tables[0].dim) if self.kind == L.MODEL_ROTATE else 0.0
+        self.neg_weight = None if neg_weight is None else float(neg_weight)
         dev = self.tables[0].device
         self.loss_dev = torch.zeros(1, dtype=torch.float64, device=dev)
         self._idx = None
@@ -403,22 +417,33 @@ class ModelTrainer:
     def _c_model(self):
         # the Table structs are owned by the EmbeddingTables (cached there), so the pointers stay valid
         ptr = lambda t: C.pointer(t.c_struct()) if t is not None else None
-        return L.Model(self.kind, *[ptr(t) for t in self.tables])
+        return L.Model(self.kind, *[ptr(t) for t in self.tables], self.gamma, self.phase)
 
-    def score_fed(self, pos, neg=None, loss_out=None, scale=None):
+    def score_fed(self, pos, neg=None, loss_out=None, scale=None, neg_scale=None):
         """pos / neg: int32 device tensors [3, n] (h | r | t rows); accumulates gradients into every table and adds
         the batch loss into loss_out (default self.loss_dev).  `scale` multiplies loss and gradient (default 1, or
-        1 / batch for `mean_loss`); it may be negative (JAPE's −α·Σ s⁻ term)."""
+        1 / batch for `mean_loss`); it may be negative (JAPE's −α·Σ s⁻ term).  `neg_scale` (default scale·neg_weight,
+        or scale when the trainer has no neg_weight) multiplies the negatives' part instead: the positives and the
+        negatives are then scored by two calls."""
         out = self.loss_dev if loss_out is None else loss_out
         n_pos = pos.shape[1]
         n_neg = 0 if neg is None else neg.shape[1]
         if scale is None:
             scale = 1.0 / max(1, n_pos + n_neg) if self.mean_loss else 1.0
+        if neg_scale is None and self.neg_weight is not None:
+            neg_scale = scale * self.neg_weight
         np_ = lambda t, i: C.c_void_p(0 if t is None or t.shape[1] == 0 else t[i].data_ptr())
         model = self._c_model()
-        L.check(self.lib.oea_model_score_fed(
-            C.byref(model), np_(pos, 0), np_(pos, 1), np_(pos, 2), n_pos, np_(neg, 0), np_(neg, 1), np_(neg, 2), n_neg,
-            C.byref(self.loss), scale, _ptr(out), _stream_ptr()), "oea_model_score_fed")
+
+        def call(p, n_p, n, n_n, s):
+            L.check(self.lib.oea_model_score_fed(
+                C.byref(model), np_(p, 0), np_(p, 1), np_(p, 2), n_p, np_(n, 0), np_(n, 1), np_(n, 2), n_n,
+                C.byref(self.loss), s, _ptr(out), _stream_ptr()), "oea_model_score_fed")
+        if neg_scale is None or n_neg == 0 or neg_scale == scale:
+            call(pos, n_pos, neg, n_neg, scale)
+        else:
+            call(pos, n_pos, None, 0, scale)
+            call(None, 0, neg, n_neg, neg_scale)
 
     def apply(self):
         for tab in self.live:

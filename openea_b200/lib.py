@@ -17,6 +17,7 @@ WEIGHT_DIRECT, WEIGHT_RECIPROCAL = 0, 1
 METRIC_INNER, METRIC_L1, METRIC_L2 = 0, 1, 2
 P2P_MAX_WORLD = 16
 MODEL_TRANSE, MODEL_TRANSH, MODEL_TRANSD, MODEL_DISTMULT, MODEL_SIMPLE = 0, 1, 2, 3, 4
+MODEL_ROTATE, MODEL_HOLE = 5, 6
 
 
 class OeaError(RuntimeError):
@@ -86,7 +87,9 @@ class SeedXchg(C.Structure):
 
 
 class Model(C.Structure):
-    _fields_ = [("kind", C.c_int32), ("ent", _TP), ("rel", _TP), ("ent_aux", _TP), ("rel_aux", _TP)]
+    # gamma / phase: RotatE's model constants (0 and ignored for the other kinds)
+    _fields_ = [("kind", C.c_int32), ("ent", _TP), ("rel", _TP), ("ent_aux", _TP), ("rel_aux", _TP),
+                ("gamma", C.c_float), ("phase", C.c_float)]
 
 
 # name → (restype, argtypes).  Must list every symbol include/oea.h declares (tests check this).

@@ -1,6 +1,4 @@
 from openea_b200.models.semantic.distmult import DistMult
+from openea_b200.models.semantic.hole import HolE
+from openea_b200.models.semantic.rotate import RotatE
 from openea_b200.models.semantic.simple import SimplE
-from openea_b200.models._stubs import out_of_scope
-
-HolE = out_of_scope("HolE", "FFT circular correlation")
-RotatE = out_of_scope("RotatE", "float64 complex rotation")

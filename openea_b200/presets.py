@@ -93,6 +93,34 @@ def distmult(scale="15K"):
     return a
 
 
+def rotate(scale="15K"):
+    """run/args/rotate_args_*.json."""
+    small = scale == "15K"
+    return _args(embedding_module="RotatE", alignment_module="sharing", dim=100, init="uniform", ent_l2_norm=True,
+                 rel_l2_norm=True, neg_sampling="uniform", neg_triple_num=10, gamma=12.0, learning_rate=0.1,
+                 optimizer="Adam", batch_size=5000 if small else 20000, batch_threads_num=2 if small else 3,
+                 test_threads_num=2 if small else 1, start_valid=200, eval_metric="inner", eval_norm=True)
+
+
+def hole(scale="15K"):
+    """run/args/hole_args_*.json."""
+    small = scale == "15K"
+    return _args(embedding_module="HolE", alignment_module="sharing", dim=100, init="xavier", ent_l2_norm=True,
+                 rel_l2_norm=True, loss_norm="L2", margin=0.2, neg_sampling="uniform", neg_triple_num=1,
+                 learning_rate=0.01, optimizer="Adagrad", batch_size=5000 if small else 20000,
+                 batch_threads_num=2 if small else 3, test_threads_num=3 if small else 10, eval_metric="inner",
+                 eval_norm=False)
+
+
+def bootea_rotate(scale="15K"):
+    """run/args/bootea_rotate_args_15K.json (the reference ships the 15K configuration only)."""
+    return _args(embedding_module="BootEA_RotatE", alignment_module="swapping", dim=100, init="normal", ent_l2_norm=True,
+                 rel_l2_norm=False, gamma=12.0, learning_rate=0.01, optimizer="Adam", batch_size=5000, min_iter=40,
+                 neg_sampling="uniform", neg_triple_num=10, truncated_epsilon=0.9, truncated_freq=10,
+                 batch_threads_num=4, test_threads_num=4, start_valid=10, start_bp=5000, eval_metric="inner",
+                 eval_norm=True, sim_th=0.75, k=10, sub_epoch=10, align_times=1)
+
+
 def bootea_transh(scale="15K"):
     a = bootea(scale)
     a.embedding_module = "BootEA_TransH"
