@@ -161,12 +161,14 @@ inline int grid_for(int n_warp_items) {
     return blocks_needed < 1 ? 1 : (blocks_needed < cap ? blocks_needed : cap);
 }
 
-// Exactly one resident wave for kernel `fn` (grid-stride loops do the rest): a partial last wave would run at a
-// fraction of the machine for a whole block duration.
-template <typename Fn>
-static int grid_one_wave(Fn fn, int n_warp_items, int warps_per_block = kWarpsPerBlock) {
-    static int occ = 0;   // one static per kernel instantiation
-    if (occ == 0 && (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, warps_per_block * OEA_WARP, 0) != cudaSuccess || occ < 1)) occ = 1;
+// Exactly one resident wave for kernel `K` (grid-stride loops do the rest): a partial last wave would run at a
+// fraction of the machine for a whole block duration.  The kernel is a template argument, not a parameter, so every
+// kernel has its own cached occupancy: kernels with the same parameter list but different launch bounds (the duo and
+// octet sampled steps) must not share one, or a cooperative launch could ask for more CTAs than can be co-resident.
+template <auto K>
+static int grid_one_wave(int n_warp_items, int warps_per_block = kWarpsPerBlock) {
+    static int occ = 0;   // one static per kernel
+    if (occ == 0 && (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, K, warps_per_block * OEA_WARP, 0) != cudaSuccess || occ < 1)) occ = 1;
     const int blocks_needed = (n_warp_items + warps_per_block - 1) / warps_per_block;
     const int cap = sm_count_cached() * occ;
     return blocks_needed < 1 ? 1 : (blocks_needed < cap ? blocks_needed : cap);

@@ -675,9 +675,9 @@ extern "C" int oea_triple_score_fed(const oea_table* ent, const oea_table* rel,
 #undef CALL
     } else {
 #define CALL(V)                                                                                                         \
-        if (l1) { const int grid = grid_one_wave(k_score_fed<OEA_SCORE_L1, V>, n_pos + n_neg);                              \
+        if (l1) { const int grid = grid_one_wave<k_score_fed<OEA_SCORE_L1, V>>(n_pos + n_neg);                              \
                   OEA_LAUNCH((k_score_fed<OEA_SCORE_L1, V>), grid, kThreads, 0, st, e, r, pos_h, pos_r, pos_t, n_pos, neg_h, neg_r, neg_t, n_neg, *loss, loss_out); } \
-        else { const int grid = grid_one_wave(k_score_fed<OEA_SCORE_L2SQ, V>, n_pos + n_neg);                               \
+        else { const int grid = grid_one_wave<k_score_fed<OEA_SCORE_L2SQ, V>>(n_pos + n_neg);                               \
                OEA_LAUNCH((k_score_fed<OEA_SCORE_L2SQ, V>), grid, kThreads, 0, st, e, r, pos_h, pos_r, pos_t, n_pos, neg_h, neg_r, neg_t, n_neg, *loss, loss_out); }
         OEA_DISPATCH_VEC(ent->pitch, CALL);
 #undef CALL
@@ -761,16 +761,16 @@ extern "C" int oea_triple_score_sampled(const oea_table* ent, const oea_table* r
     const bool l1 = loss->score_kind == OEA_SCORE_L1;
     if (!l1 && ent->pitch <= 128 && !oea_force_v1() && oea_use_duo(P.k)) {
         const int pairs = ((n_pos + P.shard_world - 1) / P.shard_world + 1) / 2;
-        const int grid = grid_one_wave(k_score_sampled_duo, pairs, kDuoWarps);
+        const int grid = grid_one_wave<k_score_sampled_duo>(pairs, kDuoWarps);
         OEA_LAUNCH(k_score_sampled_duo, grid, kDuoThreads, 0, st, e, r, P, *loss, loss_out, dbg_neg);
     } else if (!l1 && ent->pitch <= 128 && !oea_force_v1()) {
-        const int grid = grid_one_wave(k_score_sampled_oct, (n_pos + P.shard_world - 1) / P.shard_world, kOctWarps);
+        const int grid = grid_one_wave<k_score_sampled_oct>((n_pos + P.shard_world - 1) / P.shard_world, kOctWarps);
         OEA_LAUNCH(k_score_sampled_oct, grid, kOctThreads, 0, st, e, r, P, *loss, loss_out, dbg_neg);
     } else {
 #define CALL(V)                                                                                              \
-    if (l1) { const int grid = grid_one_wave(k_score_sampled<OEA_SCORE_L1, V>, (n_pos + P.shard_world - 1) / P.shard_world);                     \
+    if (l1) { const int grid = grid_one_wave<k_score_sampled<OEA_SCORE_L1, V>>((n_pos + P.shard_world - 1) / P.shard_world);                     \
               OEA_LAUNCH((k_score_sampled<OEA_SCORE_L1, V>), grid, kThreads, 0, st, e, r, P, *loss, loss_out, dbg_neg); } \
-    else { const int grid = grid_one_wave(k_score_sampled<OEA_SCORE_L2SQ, V>, (n_pos + P.shard_world - 1) / P.shard_world);                      \
+    else { const int grid = grid_one_wave<k_score_sampled<OEA_SCORE_L2SQ, V>>((n_pos + P.shard_world - 1) / P.shard_world);                      \
            OEA_LAUNCH((k_score_sampled<OEA_SCORE_L2SQ, V>), grid, kThreads, 0, st, e, r, P, *loss, loss_out, dbg_neg); }
         OEA_DISPATCH_VEC(ent->pitch, CALL);
 #undef CALL
@@ -1169,19 +1169,19 @@ extern "C" int oea_triple_step_sampled(const oea_table* ent, const oea_table* re
     if (oea_use_duo(P.k)) {
         const int pairs = (n_pos + 1) / 2;
         if (opt->kind == OEA_OPT_ADAGRAD) {
-            const int grid = grid_one_wave(k_step_sampled_duo<OEA_OPT_ADAGRAD>, pairs, kDuoWarps);
+            const int grid = grid_one_wave<k_step_sampled_duo<OEA_OPT_ADAGRAD>>(pairs, kDuoWarps);
             OEA_CUDA_TRY(OEA_LAUNCH_COOPERATIVE(k_step_sampled_duo<OEA_OPT_ADAGRAD>, grid, kDuoThreads, st, e, r, P, cfg, loss_out, A, B, lr));
         } else {
-            const int grid = grid_one_wave(k_step_sampled_duo<OEA_OPT_SGD>, pairs, kDuoWarps);
+            const int grid = grid_one_wave<k_step_sampled_duo<OEA_OPT_SGD>>(pairs, kDuoWarps);
             OEA_CUDA_TRY(OEA_LAUNCH_COOPERATIVE(k_step_sampled_duo<OEA_OPT_SGD>, grid, kDuoThreads, st, e, r, P, cfg, loss_out, A, B, lr));
         }
         return OEA_OK;
     }
     if (opt->kind == OEA_OPT_ADAGRAD) {
-        const int grid = grid_one_wave(k_step_sampled_oct<OEA_OPT_ADAGRAD>, n_pos, kOctWarps);
+        const int grid = grid_one_wave<k_step_sampled_oct<OEA_OPT_ADAGRAD>>(n_pos, kOctWarps);
         OEA_CUDA_TRY(OEA_LAUNCH_COOPERATIVE(k_step_sampled_oct<OEA_OPT_ADAGRAD>, grid, kOctThreads, st, e, r, P, cfg, loss_out, A, B, lr));
     } else {
-        const int grid = grid_one_wave(k_step_sampled_oct<OEA_OPT_SGD>, n_pos, kOctWarps);
+        const int grid = grid_one_wave<k_step_sampled_oct<OEA_OPT_SGD>>(n_pos, kOctWarps);
         OEA_CUDA_TRY(OEA_LAUNCH_COOPERATIVE(k_step_sampled_oct<OEA_OPT_SGD>, grid, kOctThreads, st, e, r, P, cfg, loss_out, A, B, lr));
     }
     return OEA_OK;

@@ -232,7 +232,7 @@ extern "C" int oea_triple_score_fed_grouped(const oea_table* ent, const oea_tabl
     const bool l1 = loss->score_kind == OEA_SCORE_L1;
     if (!l1 && ent->pitch <= 128 && oea_use_duo(k)) {
         FedBatch F{pos_h, pos_r, pos_t, neg_h, neg_r, neg_t, n_pos, k};
-        const int grid = grid_one_wave(k_score_fed_duo, (n_pos + 1) / 2, kDuoWarps);
+        const int grid = grid_one_wave<k_score_fed_duo>((n_pos + 1) / 2, kDuoWarps);
         OEA_LAUNCH(k_score_fed_duo, grid, kDuoThreads, 0, (cudaStream_t)stream, e, r, F, *loss, loss_out);
         OEA_LAUNCH_CHECK();
         return OEA_OK;
@@ -277,16 +277,16 @@ extern "C" int oea_triple_step_fed_grouped(const oea_table* ent, const oea_table
     if (ent->pitch <= 128 && oea_use_duo(k)) {
         FedBatch F{pos_h, pos_r, pos_t, neg_h, neg_r, neg_t, n_pos, k};
         if (opt->kind == OEA_OPT_ADAGRAD) {
-            const int grid = grid_one_wave(k_step_fed_duo<OEA_OPT_ADAGRAD>, (n_pos + 1) / 2, kDuoWarps);
+            const int grid = grid_one_wave<k_step_fed_duo<OEA_OPT_ADAGRAD>>((n_pos + 1) / 2, kDuoWarps);
             OEA_CUDA_TRY(OEA_LAUNCH_COOPERATIVE(k_step_fed_duo<OEA_OPT_ADAGRAD>, grid, kDuoThreads, st, e, r, F, cfg, loss_out, A, B, lr));
         } else {
-            const int grid = grid_one_wave(k_step_fed_duo<OEA_OPT_SGD>, (n_pos + 1) / 2, kDuoWarps);
+            const int grid = grid_one_wave<k_step_fed_duo<OEA_OPT_SGD>>((n_pos + 1) / 2, kDuoWarps);
             OEA_CUDA_TRY(OEA_LAUNCH_COOPERATIVE(k_step_fed_duo<OEA_OPT_SGD>, grid, kDuoThreads, st, e, r, F, cfg, loss_out, A, B, lr));
         }
         return OEA_OK;
     }
 #define OEA_RUN_STEP(V, KIND)                                                                                            \
-    do { const int grid = grid_one_wave(k_step_fed_grouped<OEA_SCORE_L2SQ, V, KIND>, n_pos);                             \
+    do { const int grid = grid_one_wave<k_step_fed_grouped<OEA_SCORE_L2SQ, V, KIND>>(n_pos);                             \
          OEA_CUDA_TRY(OEA_LAUNCH_COOPERATIVE((k_step_fed_grouped<OEA_SCORE_L2SQ, V, KIND>), grid, kThreads, st, e, r, pos_h, pos_r, \
                                              pos_t, np, neg_h, neg_r, neg_t, k, cfg, loss_out, A, B, lr)); } while (0)
     if (ent->pitch <= 128) { if (opt->kind == OEA_OPT_ADAGRAD) OEA_RUN_STEP(1, OEA_OPT_ADAGRAD); else OEA_RUN_STEP(1, OEA_OPT_SGD); }

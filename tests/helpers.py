@@ -5,10 +5,11 @@ import torch
 
 
 def torch_triple_loss(ent, rel, pos, neg, loss, loss_norm, ent_norm, rel_norm, margin=0.0, neg_margin=0.0,
-                      balance=1.0, dtype=torch.float64):
-    """Formulas of modules/base/losses.py + initializers.py:26 in torch; returns (loss, g_ent, g_rel, scores)."""
-    E = torch.tensor(np.asarray(ent), dtype=dtype, requires_grad=True)
-    R = torch.tensor(np.asarray(rel), dtype=dtype, requires_grad=True)
+                      balance=1.0, dtype=torch.float64, device="cpu"):
+    """Formulas of modules/base/losses.py + initializers.py:26 in torch; returns (loss, g_ent, g_rel, scores) as host
+    arrays.  `device` is where the float64 graph runs (a GPU makes 10⁵-triple batches cheap)."""
+    E = torch.tensor(np.asarray(ent), dtype=dtype, device=device, requires_grad=True)
+    R = torch.tensor(np.asarray(rel), dtype=dtype, device=device, requires_grad=True)
 
     def l2n(x):
         ss = (x * x).sum(1, keepdim=True)
@@ -18,12 +19,12 @@ def torch_triple_loss(ent, rel, pos, neg, loss, loss_norm, ent_norm, rel_norm, m
     Rh = l2n(R) if rel_norm else R
 
     def score(hrt):
-        hrt = torch.as_tensor(np.asarray(hrt), dtype=torch.long)
+        hrt = torch.as_tensor(np.asarray(hrt), dtype=torch.long, device=device)
         u = Eh[hrt[0]] + Rh[hrt[1]] - Eh[hrt[2]]
         return u.abs().sum(1) if loss_norm == "L1" else (u * u).sum(1)
 
     sp = score(pos)
-    sn = score(neg) if neg is not None and np.asarray(neg).size else torch.zeros(0, dtype=dtype)
+    sn = score(neg) if neg is not None and np.asarray(neg).size else torch.zeros(0, dtype=dtype, device=device)
     relu = torch.nn.functional.relu
     if loss == "margin-based":
         val = relu(margin + sp - sn).sum()
@@ -40,7 +41,7 @@ def torch_triple_loss(ent, rel, pos, neg, loss, loss_norm, ent_norm, rel_norm, m
     val.backward()
     g_e = E.grad if E.grad is not None else torch.zeros_like(E)
     g_r = R.grad if R.grad is not None else torch.zeros_like(R)
-    return float(val.detach()), g_e.numpy(), g_r.numpy(), torch.cat([sp, sn]).detach().numpy()
+    return float(val.detach()), g_e.cpu().numpy(), g_r.cpu().numpy(), torch.cat([sp, sn]).detach().cpu().numpy()
 
 
 def make_tables(rng, n_ent, n_rel, d, scale=1.0):
