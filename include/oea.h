@@ -421,14 +421,17 @@ int oea_matrix_rank(const float* mat, int64_t ld, int32_t n_rows, int32_t n_cols
  * out[n_top] = Σ(rank+1), out[n_top+1] = Σ 1/(rank+1); device fp64 [n_top + 2], zeroed here. top_k_host is a HOST array. */
 int oea_rank_stats(const int32_t* rank, int32_t n, const int32_t* top_k_host, int32_t n_top, double* out, void* stream);
 
-/* sklearn.preprocessing.normalize (similarity.py:30-32): rows scaled to unit L2 norm, zero rows kept;
- * writes zero padding up to out_pitch. */
+/* sklearn.preprocessing.normalize (similarity.py:30-32) with the rule of scikit-learn >= 1.0: rows scaled to unit L2
+ * norm, except that a row whose fp32 norm is below 10·FLT_EPSILON (a zero row, or a non-zero row whose squared norm
+ * underflows) is copied unchanged; writes zero padding up to out_pitch. */
 int oea_rows_normalize(const float* in, int32_t in_pitch, int32_t n, int32_t dim, float* out, int32_t out_pitch,
                        void* stream);
 
 /* Per-row k LARGEST entries of a materialised matrix, large k (the ε-truncated neighbour search,
- * modules/train/batch.py:157-165: np.argpartition(-sim, k)[:k]); only SET membership is defined.
- * out_idx [n_rows, k] = col_ids[column] (col_ids == NULL → the column index itself). */
+ * modules/train/batch.py:157-165: np.argpartition(-sim, k)[:k]).  The set is the first k columns by (value
+ * descending, column ascending): of the columns tied at the k-th value the lowest-index ones are taken.  Each row of
+ * out_idx [n_rows, k] lists that set in ascending column order, as col_ids[column] (col_ids == NULL → the column
+ * index itself); the output is deterministic.  oea_rows_gather_sort orders it by value. */
 int oea_rows_select_topk(const float* mat, int64_t ld, int32_t n_rows, int32_t n_cols, int32_t k,
                          const int32_t* col_ids, int32_t* out_idx, void* stream);
 

@@ -454,7 +454,9 @@ __global__ void k_rank_finish(const unsigned long long* __restrict__ best, int n
     if (i < n1) top1[i] = 0x7fffffff - (int)(best[i] & 0xffffffffu);
 }
 
-// sklearn.preprocessing.normalize(x) (similarity.py:30-32): x / ||x||₂, zero rows stay zero.
+// sklearn.preprocessing.normalize(x) (similarity.py:30-32): x / ||x||₂.  The rule of scikit-learn ≥ 1.0
+// (_handle_zeros_in_scale): a row whose fp32 norm is below 10·FLT_EPSILON is left unchanged, and that includes a zero
+// row and a non-zero row whose squared norm underflows to 0.  (scikit-learn < 1.0 normalised every non-zero row.)
 __global__ void __launch_bounds__(256)
 k_rows_normalize(const float* __restrict__ in, int in_pitch, int n, int dim, float* __restrict__ out, int out_pitch) {
     const int lane = threadIdx.x & 31;
@@ -464,7 +466,8 @@ k_rows_normalize(const float* __restrict__ in, int in_pitch, int n, int dim, flo
     float ss = 0.f;
     for (int c = lane; c < dim; c += 32) { const float x = src[c]; ss = fmaf(x, x, ss); }
     ss = warp_sum(ss);
-    const float inv = ss > 0.f ? 1.f / sqrtf(ss) : 0.f;
+    const float nrm = sqrtf(ss);
+    const float inv = nrm < 10.f * FLT_EPSILON ? 1.f : 1.f / nrm;
     float* dst = out + (size_t)row * out_pitch;
     for (int c = lane; c < out_pitch; c += 32) dst[c] = c < dim ? src[c] * inv : 0.f;
 }
@@ -710,8 +713,9 @@ extern "C" int oea_rows_normalize(const float* in, int32_t in_pitch, int32_t n, 
 
 // ------------------------------------------------------------------------------------------------
 // Large-k per-row selection (ε-truncated neighbour search): 3-pass MSB radix select (11+11+10 bits)
-// on the order-preserving integer image of the floats, then one compaction pass.  One CTA per row;
-// passes 2-4 re-read the row from L2.
+// on the order-preserving integer image of the floats, then one ordered compaction pass.  One CTA per row;
+// passes 2-4 re-read the row from L2.  The selected set is the first k columns by (value descending, index
+// ascending): of the columns equal to the threshold, the lowest-index ones.  It is written in ascending column order.
 // ------------------------------------------------------------------------------------------------
 namespace oea {
 
@@ -722,17 +726,20 @@ __device__ __forceinline__ unsigned fkey(float f) {
 
 constexpr int SEL_THREADS = 512;
 constexpr int SEL_BINS = 2048;
+constexpr int SEL_CPT = 8;        // consecutive columns per thread in the compaction pass (multiple of 4)
 
 __global__ void __launch_bounds__(SEL_THREADS)
 k_rows_select(const float* __restrict__ mat, long long ld, int n_rows, int n_cols, int k,
               const int32_t* __restrict__ col_ids, int32_t* __restrict__ out) {
     __shared__ unsigned hist[SEL_BINS];
     __shared__ unsigned s_chunk[32];
-    __shared__ unsigned s_prefix, s_mask, s_remaining, s_gt, s_eq;
+    __shared__ unsigned s_warp[SEL_THREADS / 32];
+    __shared__ unsigned s_prefix, s_mask, s_remaining;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const bool vec = (ld & 3) == 0 && aligned16(mat);      // 16-B loads in the compaction pass
     for (int row = blockIdx.x; row < n_rows; row += gridDim.x) {
         const float* src = mat + (size_t)row * ld;
-        if (tid == 0) { s_prefix = 0u; s_mask = 0u; s_remaining = (unsigned)k; s_gt = 0u; s_eq = 0u; }
+        if (tid == 0) { s_prefix = 0u; s_mask = 0u; s_remaining = (unsigned)k; }
         __syncthreads();
 #pragma unroll 1
         for (int pass = 0; pass < 3; ++pass) {
@@ -776,19 +783,61 @@ k_rows_select(const float* __restrict__ mat, long long ld, int n_rows, int n_col
             __syncthreads();
         }
         const unsigned T = s_prefix, take_eq = s_remaining;
-        const unsigned n_gt = (unsigned)k - take_eq;
         int32_t* dst = out + (size_t)row * k;
-        for (int j = tid; j < n_cols; j += SEL_THREADS) {
-            const unsigned u = fkey(__ldg(src + j));
-            if (u > T) {
-                const unsigned p = atomicAdd(&s_gt, 1u);
-                dst[p] = col_ids ? __ldg(col_ids + j) : j;
-            } else if (u == T) {
-                const unsigned e = atomicAdd(&s_eq, 1u);
-                if (e < take_eq) dst[n_gt + e] = col_ids ? __ldg(col_ids + j) : j;
+        // ordered compaction, one chunk of SEL_CPT·512 columns at a time (SEL_CPT consecutive columns per thread): a block
+        // scan of the packed counts (above T) << 16 | (== T) gives each column the number of selected columns before
+        // it, #above + min(#equal, take_eq)
+        unsigned gt_base = 0, eq_base = 0;          // totals of the chunks already done (the same in every thread)
+        for (int j0 = 0; j0 < n_cols; j0 += SEL_CPT * SEL_THREADS) {
+            const int j = j0 + SEL_CPT * tid;
+            unsigned flag[SEL_CPT];                 // per column: 0x10000 above T, 1 equal to T, 0 otherwise
+#pragma unroll
+            for (int q = 0; q < SEL_CPT; q += 4) {
+                float v[4];
+                if (vec && j + q + 3 < n_cols) {
+                    const float4 t = ldg4(src + j + q);
+                    v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+                } else {
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) v[e] = j + q + e < n_cols ? __ldg(src + j + q + e) : 0.f;
+                }
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const unsigned u = fkey(v[e]);
+                    flag[q + e] = j + q + e >= n_cols ? 0u : (u > T ? 0x10000u : (u == T ? 1u : 0u));
+                }
             }
+            unsigned f = 0;                         // per-chunk counts are ≤ SEL_CPT·512 < 2^16: 16 bits each
+#pragma unroll
+            for (int q = 0; q < SEL_CPT; ++q) f += flag[q];
+            unsigned incl = f;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const unsigned y = __shfl_up_sync(OEA_FULL, incl, o);
+                if (lane >= o) incl += y;
+            }
+            if (lane == 31) s_warp[warp] = incl;
+            __syncthreads();
+            unsigned before = 0, total = 0;
+#pragma unroll
+            for (int w = 0; w < SEL_THREADS / 32; ++w) {
+                const unsigned t = s_warp[w];
+                before += w < warp ? t : 0u;
+                total += t;
+            }
+            __syncthreads();                        // s_warp is rewritten by the next chunk
+            unsigned excl = before + incl - f;
+#pragma unroll
+            for (int q = 0; q < SEL_CPT; ++q) {
+                const unsigned eq_before = eq_base + (excl & 0xffffu);
+                if (flag[q] == 0x10000u || (flag[q] == 1u && eq_before < take_eq))
+                    dst[gt_base + (excl >> 16) + min(eq_before, take_eq)] = col_ids ? __ldg(col_ids + j + q) : j + q;
+                excl += flag[q];
+            }
+            gt_base += total >> 16;
+            eq_base += total & 0xffffu;
+            if (gt_base + min(eq_base, take_eq) == (unsigned)k) break;   // uniform: every thread holds the same totals
         }
-        __syncthreads();
     }
 }
 

@@ -11,10 +11,11 @@ import numpy as np
 
 
 def normalize_rows(x):
-    """sklearn.preprocessing.normalize (similarity.py:30-32): unit L2 rows, zero rows unchanged."""
+    """sklearn.preprocessing.normalize (similarity.py:30-32) as scikit-learn >= 1.0 does it: unit L2 rows; a row whose
+    float32 norm is below 10·eps (a zero row, or one whose squared norm underflows) is left unchanged."""
     x = np.asarray(x, dtype=np.float32)
     n = np.sqrt((x.astype(np.float32) ** 2).sum(1, keepdims=True))
-    n[n == 0] = 1.0
+    n[n < 10 * np.finfo(np.float32).eps] = 1.0
     return (x / n).astype(np.float32)
 
 
