@@ -249,16 +249,21 @@ int oea_triple_step_fed_host(const oea_table* ent, const oea_table* rel,
  * softplus(−score⁺) + softplus(score⁻).  ROTATE's energy is the distance minus γ, so OEA_LOSS_LOGISTIC is the reference's
  * −log σ(γ − d⁺) − log σ(d⁻ − γ) and OEA_LOSS_LOGSIGMOID its alignment loss −log σ(γ − d).
  * ROTATE and HOLE run in fp32 like every other kind (the reference keeps RotatE's variables in float64); the gradient of
- * RotatE's modulus at a zero coordinate is 0 (TF's is NaN there).  HOLE computes the correlation directly, O(dim²). */
+ * RotatE's modulus at a zero coordinate is 0 (TF's is NaN there).  HOLE computes the correlation directly, O(dim²).
+ *   TRANSR    Σ|l2n(M_r·ĥ) + r̂ − l2n(M_r·t̂)| or Σ(·)², M_r = rel_matrix[r] as d×d     models/trans/transr.py:14-52
+ *             (row-major).  The projections are l2-normalised whatever ent's l2_norm says; the matrix never is.  rel_aux
+ *             is the matrix table: rows = rel->rows·dim, row r·dim + i = row i of M_r.  Scored by oea_transr_score_fed
+ *             only (it needs a workspace); oea_model_score_fed returns OEA_ERR_KIND for it. */
 enum { OEA_MODEL_TRANSE = 0, OEA_MODEL_TRANSH = 1, OEA_MODEL_TRANSD = 2, OEA_MODEL_DISTMULT = 3, OEA_MODEL_SIMPLE = 4,
-       OEA_MODEL_ROTATE = 5, OEA_MODEL_HOLE = 6 };
+       OEA_MODEL_ROTATE = 5, OEA_MODEL_HOLE = 6, OEA_MODEL_TRANSR = 7 };
 
 typedef struct oea_model {
     int32_t kind;              /* OEA_MODEL_* */
     const oea_table* ent;      /* ent_embeds                                 | SIMPLE: head_ent_embeds | ROTATE: re_ent_embeds */
     const oea_table* rel;      /* rel_embeds                                 | SIMPLE: rel_embeds1 */
     const oea_table* ent_aux;  /* TRANSD: ent_transfer | SIMPLE: tail_ent_embeds | ROTATE: im_ent_embeds | else NULL */
-    const oea_table* rel_aux;  /* TRANSH: normal_vector, TRANSD: rel_transfer | SIMPLE: rel_embeds2   | else NULL */
+    const oea_table* rel_aux;  /* TRANSH: normal_vector, TRANSD: rel_transfer | SIMPLE: rel_embeds2   | TRANSR: rel_matrix
+                                * | else NULL */
     float gamma;               /* ROTATE: γ (args.gamma); ignored by the other kinds */
     float phase;               /* ROTATE: π/ρ with ρ = (γ + 2)/dim, the scale from r̂ to the phase (rotate.py:37,90);
                                 * ignored by the other kinds */
@@ -277,6 +282,21 @@ int oea_model_score_fed(const oea_model* model,
                         const int32_t* pos_h, const int32_t* pos_r, const int32_t* pos_t, int32_t n_pos,
                         const int32_t* neg_h, const int32_t* neg_r, const int32_t* neg_t, int32_t n_neg,
                         const oea_loss_cfg* loss, float loss_scale, double* loss_out, void* stream);
+
+/* TransR's fed step (models/trans/transr.py:14-52), with oea_model_score_fed's semantics, loss kinds, pairing rule and
+ * argument checks, for model->kind == OEA_MODEL_TRANSR: the scored triples are grouped by relation on the device, and
+ * each chunk of ≤ 64 triples of one relation reads M_r once and reduces its gradient once (red into rel_aux->grad,
+ * its d rows flagged in rel_aux->touched).  Entity and relation gradients as every other kind.  FP32 throughout.
+ * OEA_ERR_DIM when pitch > 128 or the three tables disagree on pitch; OEA_ERR_SHAPE when rel_aux->rows != rel->rows·dim
+ * or rel_aux->dim != dim; OEA_ERR_WORKSPACE when the 16-byte aligned workspace is smaller than
+ * oea_transr_workspace_bytes(n_pos, n_neg, dim, rel->rows).  No allocation, no host synchronisation.
+ * Run oea_rowopt_apply on the three tables afterwards. */
+size_t oea_transr_workspace_bytes(int32_t n_pos, int32_t n_neg, int32_t dim, int32_t n_rel);
+int oea_transr_score_fed(const oea_model* model,
+                         const int32_t* pos_h, const int32_t* pos_r, const int32_t* pos_t, int32_t n_pos,
+                         const int32_t* neg_h, const int32_t* neg_r, const int32_t* neg_t, int32_t n_neg,
+                         const oea_loss_cfg* loss, float loss_scale, void* workspace, size_t workspace_bytes,
+                         double* loss_out, void* stream);
 
 /* The batch producer of modules/train/batch.py:36-45 (generate_relation_triple_batch) / :168-184
  * (generate_triple_label_batch) on the device: writes the index vectors a fed step takes.

@@ -136,6 +136,96 @@ __host__ inline TableDev table_dev(const oea_table* t) {
     return d;
 }
 
+// ---- whole-row arithmetic (oea_triple_ext.cu, oea_triple_transr.cu) ------------------------------------------
+__device__ __forceinline__ float4 mul4(float4 a, float4 b) { return cat4(mul2(lo2(a), lo2(b)), mul2(hi2(a), hi2(b))); }
+
+template <int VEC>
+__device__ __forceinline__ Row<VEC> r_scale(const Row<VEC>& a, float s) {
+    Row<VEC> o;
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) o.v[i] = a.v[i] * s;
+    return o;
+}
+template <int VEC>
+__device__ __forceinline__ Row<VEC> r_add(const Row<VEC>& a, const Row<VEC>& b) {
+    Row<VEC> o;
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) o.v[i] = a.v[i] + b.v[i];
+    return o;
+}
+template <int VEC>
+__device__ __forceinline__ Row<VEC> r_sub(const Row<VEC>& a, const Row<VEC>& b) {
+    Row<VEC> o;
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) o.v[i] = a.v[i] - b.v[i];
+    return o;
+}
+template <int VEC>
+__device__ __forceinline__ Row<VEC> r_neg(const Row<VEC>& a) {
+    Row<VEC> o;
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) o.v[i] = neg(a.v[i]);
+    return o;
+}
+// a·s + c
+template <int VEC>
+__device__ __forceinline__ Row<VEC> r_fma(const Row<VEC>& a, float s, const Row<VEC>& c) {
+    Row<VEC> o;
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) o.v[i] = fma4(a.v[i], s, c.v[i]);
+    return o;
+}
+// element-wise product
+template <int VEC>
+__device__ __forceinline__ Row<VEC> r_mul(const Row<VEC>& a, const Row<VEC>& b) {
+    Row<VEC> o;
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) o.v[i] = mul4(a.v[i], b.v[i]);
+    return o;
+}
+
+// A normalised row together with what the backward through l2_normalize needs.
+template <int VEC>
+struct NRow {
+    Row<VEC> x;   // x·rsqrt(max(Σx², eps)) (or x itself when the normalisation is off)
+    float inv;    // the scale that was applied
+    float ss;     // Σx² of the un-normalised row
+};
+
+// tf.nn.embedding_lookup(init_embeddings(..., is_l2_norm), row)
+template <int VEC>
+__device__ __forceinline__ NRow<VEC> lookup(const TableDev& T, int row, int lane) {
+    NRow<VEC> r;
+    r.x = load_row<VEC>(T.w, row, T.pitch, lane);
+    r.ss = warp_sum(sumsq(r.x));
+    r.inv = inv_norm(r.ss, T.norm);
+    r.x = r_scale(r.x, r.inv);
+    return r;
+}
+// tf.nn.l2_normalize of a computed row
+template <int VEC>
+__device__ __forceinline__ NRow<VEC> normalised(const Row<VEC>& v) {
+    NRow<VEC> r;
+    r.ss = warp_sum(sumsq(v));
+    r.inv = inv_norm(r.ss, true);
+    r.x = r_scale(v, r.inv);
+    return r;
+}
+// gradient w.r.t. the argument of normalised() given the gradient w.r.t. its result
+template <int VEC>
+__device__ __forceinline__ Row<VEC> back_normalised(const Row<VEC>& ghat, const NRow<VEC>& n) {
+    const float dot = warp_sum(dotr(n.x, ghat));
+    return through_norm(ghat, n.x, dot, n.inv, n.ss, true);
+}
+// gradient of a lookup(): through the table's normalisation, then one vector reduction into its gradient row
+template <int VEC>
+__device__ __forceinline__ void push(const TableDev& T, int row, int lane, const Row<VEC>& ghat, const NRow<VEC>& n) {
+    const float dot = warp_sum(dotr(n.x, ghat));
+    const Row<VEC> g = through_norm(ghat, n.x, dot, n.inv, n.ss, T.norm);
+    red_row<VEC>(T.g, row, T.pitch, lane, g);
+    if (lane == 0) T.touched[row] = 1;
+}
+
 // ---- host-side validation + dispatch -----------------------------------------------------------
 inline int check_table(const oea_table* t, bool need_grad) {
     if (t == nullptr || t->weight == nullptr) return OEA_ERR_NULL;

@@ -376,7 +376,8 @@ class TripleTrainer:
 
 
 MODEL_KINDS = {"TransE": L.MODEL_TRANSE, "TransH": L.MODEL_TRANSH, "TransD": L.MODEL_TRANSD,
-               "DistMult": L.MODEL_DISTMULT, "SimplE": L.MODEL_SIMPLE, "RotatE": L.MODEL_ROTATE, "HolE": L.MODEL_HOLE}
+               "DistMult": L.MODEL_DISTMULT, "SimplE": L.MODEL_SIMPLE, "RotatE": L.MODEL_ROTATE, "HolE": L.MODEL_HOLE,
+               "TransR": L.MODEL_TRANSR}
 
 ROTATE_EPSILON = 2.0      # rotate.py:25: the embedding range is (γ + ε) / dim
 
@@ -388,13 +389,14 @@ def rotate_phase(gamma, dim):
 
 class ModelTrainer:
     """Forward/backward + optimiser for the score functions beyond plain translation (oea_model_score_fed):
-    TransH / TransD / DistMult / SimplE / RotatE / HolE graphs of the reference's models/ (SURVEY §8f-2).
+    TransH / TransD / DistMult / SimplE / RotatE / HolE / TransR graphs of the reference's models/ (SURVEY §8f-2).
 
     tables = (ent, rel, ent_aux, rel_aux) EmbeddingTables in the slot order of `oea_model` (None where a model has
     no such table).  A step = device batch producer (oea_triple_sample_batch) → fed scorer → one row-optimiser
     launch per table; `mean_loss` applies DistMult's reduce_mean (distmult.py:58).  `gamma`: RotatE's γ (the phase
     scale follows from it and the dimension).  `neg_weight`: weight of the negatives' loss relative to the positives'
-    (RotatE's 1/k, rotate.py:81); None = the same weight."""
+    (RotatE's 1/k, rotate.py:81); None = the same weight.  TransR (rel_aux = the matrix table, R·d rows of width d)
+    is scored by oea_transr_score_fed, in a workspace the trainer owns and grows on demand."""
 
     def __init__(self, model, tables, loss, lr, mean_loss=False, sampler="fast", gamma=None, neg_weight=None):
         self.lib = L.load()
@@ -413,6 +415,14 @@ class ModelTrainer:
         self.loss_dev = torch.zeros(1, dtype=torch.float64, device=dev)
         self._idx = None
         self._n_pos = C.c_int32(0)
+        self._ws = None
+
+    def _workspace(self, n_pos, n_neg):
+        """TransR's scratch (bucketed triple ids, chunk list, scores, projections) for a batch of this size."""
+        need = self.lib.oea_transr_workspace_bytes(n_pos, n_neg, self.tables[0].dim, self.tables[1].rows)
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(max(1, need), dtype=torch.uint8, device=self.tables[0].device)
+        return self._ws
 
     def _c_model(self):
         # the Table structs are owned by the EmbeddingTables (cached there), so the pointers stay valid
@@ -436,6 +446,12 @@ class ModelTrainer:
         model = self._c_model()
 
         def call(p, n_p, n, n_n, s):
+            if self.kind == L.MODEL_TRANSR:
+                ws = self._workspace(n_p, n_n)
+                L.check(self.lib.oea_transr_score_fed(
+                    C.byref(model), np_(p, 0), np_(p, 1), np_(p, 2), n_p, np_(n, 0), np_(n, 1), np_(n, 2), n_n,
+                    C.byref(self.loss), s, _ptr(ws), ws.numel(), _ptr(out), _stream_ptr()), "oea_transr_score_fed")
+                return
             L.check(self.lib.oea_model_score_fed(
                 C.byref(model), np_(p, 0), np_(p, 1), np_(p, 2), n_p, np_(n, 0), np_(n, 1), np_(n, 2), n_n,
                 C.byref(self.loss), s, _ptr(out), _stream_ptr()), "oea_model_score_fed")

@@ -17,7 +17,7 @@ WEIGHT_DIRECT, WEIGHT_RECIPROCAL = 0, 1
 METRIC_INNER, METRIC_L1, METRIC_L2 = 0, 1, 2
 P2P_MAX_WORLD = 16
 MODEL_TRANSE, MODEL_TRANSH, MODEL_TRANSD, MODEL_DISTMULT, MODEL_SIMPLE = 0, 1, 2, 3, 4
-MODEL_ROTATE, MODEL_HOLE = 5, 6
+MODEL_ROTATE, MODEL_HOLE, MODEL_TRANSR = 5, 6, 7
 
 
 class OeaError(RuntimeError):
@@ -146,6 +146,9 @@ SIGNATURES = {
     "oea_tripleset_build": (C.c_int, [_P, _I, _P, C.c_uint32, C.c_uint32, C.c_uint32, _P]),
     "oea_model_score_fed": (C.c_int, [C.POINTER(Model), _P, _P, _P, _I, _P, _P, _P, _I, C.POINTER(LossCfg), C.c_float,
                                       _P, _P]),
+    "oea_transr_workspace_bytes": (C.c_size_t, [_I, _I, _I, _I]),
+    "oea_transr_score_fed": (C.c_int, [C.POINTER(Model), _P, _P, _P, _I, _P, _P, _P, _I, C.POINTER(LossCfg), C.c_float,
+                                       _P, C.c_size_t, _P, _P]),
     "oea_rows_gather_sort": (C.c_int, [_P, _L, _I, _I, _P, _P, _P]),
     "oea_gale_shapley_workspace_bytes": (C.c_size_t, [_I, _I]),
     "oea_gale_shapley": (C.c_int, [_P, _P, _I, _I, _I, _I, _P, _P, C.c_size_t, C.POINTER(C.c_int32), _P]),

@@ -1,6 +1,4 @@
 from openea_b200.models.trans.transe import TransE
 from openea_b200.models.trans.transh import TransH
 from openea_b200.models.trans.transd import TransD
-from openea_b200.models._stubs import out_of_scope
-
-TransR = out_of_scope("TransR", "per-relation projection matrices, not in BASELINE configs")
+from openea_b200.models.trans.transr import TransR

@@ -51,26 +51,48 @@ def init_embeddings(shape, name, init, is_l2_norm, dtype=None, optimizer=None):
     return None
 
 
-def xavier_init(shape, name, is_l2_norm, dtype=None, optimizer=None):
+def init_values(shape, init):
+    """The values init_embeddings(shape, name, init, ...) holds, as a host tensor of `shape`, drawn with that shape's
+    distribution (TransR draws its [R, d²] matrix table this way and stores it as R·d rows of width d)."""
+    draw = {'xavier': _xavier_values, 'normal': _normal_values, 'uniform': _uniform_values, 'unit': _unit_values}
+    if init not in draw:
+        raise ValueError("unknown init %r" % (init,))
+    return draw[init](shape)
+
+
+def _xavier_values(shape):
     # tf.contrib.layers.xavier_initializer(uniform=False): truncated normal, σ = sqrt(1.3·2/(fan_in+fan_out))
-    std = math.sqrt(1.3 * 2.0 / (shape[0] + shape[1]))
-    return _make(_trunc_normal(shape, std), is_l2_norm, optimizer)
+    return _trunc_normal(shape, math.sqrt(1.3 * 2.0 / (shape[0] + shape[1])))
+
+
+def _normal_values(shape):
+    return _trunc_normal(shape, 1.0 / math.sqrt(shape[1]))
+
+
+def _uniform_values(shape, minval=0, maxval=None):
+    hi = 1.0 if maxval is None else float(maxval)
+    return torch.rand(*shape, generator=_GEN, dtype=torch.float32) * (hi - minval) + minval
+
+
+def _unit_values(shape):
+    t = torch.randn(*shape, generator=_GEN, dtype=torch.float32)
+    return t / t.norm(dim=1, keepdim=True).clamp_min(1e-12)       # sklearn.preprocessing.normalize
+
+
+def xavier_init(shape, name, is_l2_norm, dtype=None, optimizer=None):
+    return _make(_xavier_values(shape), is_l2_norm, optimizer)
 
 
 def truncated_normal_init(shape, name, is_l2_norm, dtype=None, optimizer=None):
-    return _make(_trunc_normal(shape, 1.0 / math.sqrt(shape[1])), is_l2_norm, optimizer)
+    return _make(_normal_values(shape), is_l2_norm, optimizer)
 
 
 def random_uniform_init(shape, name, is_l2_norm, minval=0, maxval=None, dtype=None, optimizer=None):
-    hi = 1.0 if maxval is None else float(maxval)
-    t = torch.rand(*shape, generator=_GEN, dtype=torch.float32) * (hi - minval) + minval
-    return _make(t, is_l2_norm, optimizer)
+    return _make(_uniform_values(shape, minval, maxval), is_l2_norm, optimizer)
 
 
 def random_unit_init(shape, name, is_l2_norm, dtype=None, optimizer=None):
-    t = torch.randn(*shape, generator=_GEN, dtype=torch.float32)
-    t = t / t.norm(dim=1, keepdim=True).clamp_min(1e-12)       # sklearn.preprocessing.normalize
-    return _make(t, is_l2_norm, optimizer)
+    return _make(_unit_values(shape), is_l2_norm, optimizer)
 
 
 def orthogonal_init(shape, name, dtype=None, optimizer=None):

@@ -79,6 +79,14 @@ def transd(scale="15K"):
     return a
 
 
+def transr(scale="15K"):
+    """run/args/transr_args_15K.json (the reference ships the 15K configuration only)."""
+    return _args(embedding_module="TransR", alignment_module="sharing", dim=100, init="normal", ent_l2_norm=True,
+                 rel_l2_norm=True, loss_norm="L2", margin=1.5, loss="margin-based", neg_sampling="uniform",
+                 neg_triple_num=1, learning_rate=0.01, optimizer="Adagrad", batch_size=5000, batch_threads_num=2,
+                 test_threads_num=4, eval_metric="inner", eval_norm=False)
+
+
 def simple(scale="15K"):
     return _args(embedding_module="SimplE", alignment_module="sharing", dim=100, init="xavier", ent_l2_norm=True,
                  rel_l2_norm=True, learning_rate=0.01, optimizer="Adagrad", batch_size=5000 if scale == "15K" else 20000,
