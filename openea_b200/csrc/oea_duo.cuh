@@ -298,7 +298,7 @@ __device__ __forceinline__ void duo_score_body(const TableDev& ent, const TableD
                 const float sp_b = __shfl_sync(OEA_FULL, sp, b);
                 const int oct = lane >> 3;
                 const int role = oct < 3 ? oct : 2;
-                const TableDev& tab = role == 1 ? rel : ent;
+                const TableDev tab = pick_table(role == 1, rel, ent);
                 const int row = role == 0 ? eh : (role == 1 ? er : et);
                 R4 x = load_oct(tab.w, row, tab.pitch, l, p4);
                 float2 ss2 = make_float2(0.f, 0.f);
@@ -363,7 +363,7 @@ __device__ __forceinline__ void duo_score_body(const TableDev& ent, const TableD
             for (int pass = 0; pass < 2; ++pass) {
                 const int role = pass == 0 ? o2 : 2;
                 const int row = role == 0 ? h : (role == 1 ? r : t);
-                const TableDev& tab = role == 1 ? rel : ent;
+                const TableDev tab = pick_table(role == 1, rel, ent);
                 const R4 xo = load_oct(tab.w, row, tab.pitch, l, p4);                    // L1 hit
                 const float io = role == 0 ? ih : (role == 1 ? ir : it);
                 const float so = role == 0 ? ssh : (role == 1 ? ssr : sst);

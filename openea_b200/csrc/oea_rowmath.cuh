@@ -136,6 +136,15 @@ __host__ inline TableDev table_dev(const oea_table* t) {
     return d;
 }
 
+// c ? a : b, field by field.  `const TableDev& t = c ? a : b` on kernel parameters takes their addresses, which puts
+// both structs in a local-memory stack frame; choosing each field keeps the choice in registers.
+__device__ __forceinline__ TableDev pick_table(bool c, const TableDev& a, const TableDev& b) {
+    TableDev t;
+    t.w = c ? a.w : b.w; t.g = c ? a.g : b.g; t.touched = c ? a.touched : b.touched;
+    t.pitch = c ? a.pitch : b.pitch; t.norm = c ? a.norm : b.norm;
+    return t;
+}
+
 // ---- whole-row arithmetic (oea_triple_ext.cu, oea_triple_transr.cu) ------------------------------------------
 __device__ __forceinline__ float4 mul4(float4 a, float4 b) { return cat4(mul2(lo2(a), lo2(b)), mul2(hi2(a), hi2(b))); }
 

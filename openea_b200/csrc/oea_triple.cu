@@ -528,7 +528,7 @@ k_step_sampled_oct(TableDev ent, TableDev rel, const __grid_constant__ SampledPa
     __shared__ OctStage s_stage[kOctWarps];
     oct_score_body(ent, rel, P, cfg, loss_out, nullptr, s_loss, s_stage);
     cooperative_groups::this_grid().sync();
-    oct_rowopt_body<KIND>(A, B, ent.pitch, lr, blockIdx.x * kOctWarps + (threadIdx.x >> 5), gridDim.x * kOctWarps);
+    rowopt_flagged_body<KIND>(A, B, ent.pitch, lr, blockIdx.x * kOctWarps + (threadIdx.x >> 5), gridDim.x * kOctWarps);
 }
 
 // The duo scorer (oea_duo.cuh): two positives per warp, sampled source.
@@ -551,7 +551,7 @@ k_step_sampled_duo(TableDev ent, TableDev rel, const __grid_constant__ SampledPa
     FedBatch none{};
     duo_score_body<false>(ent, rel, P, none, cfg, loss_out, nullptr, s_loss, s_stage);
     cooperative_groups::this_grid().sync();
-    oct_rowopt_body<KIND>(A, B, ent.pitch, lr, blockIdx.x * kDuoWarps + (threadIdx.x >> 5), gridDim.x * kDuoWarps);
+    rowopt_flagged_body<KIND>(A, B, ent.pitch, lr, blockIdx.x * kDuoWarps + (threadIdx.x >> 5), gridDim.x * kDuoWarps);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1083,40 +1083,12 @@ extern "C" int oea_mapping_fwd_bwd(const float* e1, const float* e2, int32_t n, 
 namespace oea {
 
 
-// Adagrad / SGD over the concatenated row space [ent rows | rel rows] (same pitch), flagged rows only.
+// Adagrad / SGD over the concatenated row space [ent rows | rel rows] (same pitch), flagged rows only
+// (rowopt_flagged_body, the optimiser phase of the one-launch steps, on a grid of its own).
 template <int KIND>
 __global__ void __launch_bounds__(kThreads)
 k_rowopt_pair(OptTab A, OptTab B, int pitch, float lr) {
-    const int lane = threadIdx.x & 31;
-    const int warp_global = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
-    const int n_warps = gridDim.x * kWarpsPerBlock;
-    const int p4 = pitch >> 2;
-    const int total = A.rows + B.rows;
-    for (int r = warp_global; r < total; r += n_warps) {
-        const bool first = r < A.rows;
-        const OptTab& T = first ? A : B;
-        const int row = first ? r : r - A.rows;
-        if (T.touched[row] == 0) continue;
-        const size_t base = (size_t)row * pitch;
-        for (int c = lane; c < p4; c += OEA_WARP) {
-            const size_t o = base + 4 * (size_t)c;
-            const float4 g = *reinterpret_cast<const float4*>(T.g + o);
-            float4 x = *reinterpret_cast<float4*>(T.w + o);
-            if (KIND == OEA_OPT_ADAGRAD) {
-                float4 a = *reinterpret_cast<float4*>(T.s1 + o);
-                a.x = fmaf(g.x, g.x, a.x); a.y = fmaf(g.y, g.y, a.y); a.z = fmaf(g.z, g.z, a.z); a.w = fmaf(g.w, g.w, a.w);
-                x.x -= lr * g.x * rsqrtf(a.x); x.y -= lr * g.y * rsqrtf(a.y);
-                x.z -= lr * g.z * rsqrtf(a.z); x.w -= lr * g.w * rsqrtf(a.w);
-                *reinterpret_cast<float4*>(T.s1 + o) = a;
-            } else {
-                x.x -= lr * g.x; x.y -= lr * g.y; x.z -= lr * g.z; x.w -= lr * g.w;
-            }
-            *reinterpret_cast<float4*>(T.w + o) = x;
-            *reinterpret_cast<float4*>(T.g + o) = f4(0.f);
-        }
-        __syncwarp();      // as in k_rowopt: all lanes have read the flag before it is cleared
-        if (lane == 0) T.touched[row] = 0;
-    }
+    rowopt_flagged_body<KIND>(A, B, pitch, lr, blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5), gridDim.x * kWarpsPerBlock);
 }
 
 }  // namespace oea
@@ -1131,7 +1103,7 @@ extern "C" int oea_rowopt_apply_pair(const oea_table* a, const oea_table* b, con
     }
     if (opt->kind == OEA_OPT_ADAGRAD && (!a->state1 || !b->state1)) return OEA_ERR_NULL;
     OptTab A{a->weight, a->grad, a->state1, a->touched, a->rows}, B{b->weight, b->grad, b->state1, b->touched, b->rows};
-    const int grid = grid_for(a->rows + b->rows);
+    const int grid = grid_for((a->rows + b->rows + 3) / 4);     // a warp per quad of rows, up to the resident cap
     cudaStream_t st = (cudaStream_t)stream;
     if (opt->kind == OEA_OPT_ADAGRAD) OEA_LAUNCH(k_rowopt_pair<OEA_OPT_ADAGRAD>, grid, kThreads, 0, st, A, B, a->pitch, opt->lr);
     else if (opt->kind == OEA_OPT_SGD) OEA_LAUNCH(k_rowopt_pair<OEA_OPT_SGD>, grid, kThreads, 0, st, A, B, a->pitch, opt->lr);

@@ -185,7 +185,7 @@ k_step_fed_grouped(TableDev ent, TableDev rel,
     __shared__ double s_loss[kWarpsPerBlock];
     grouped_score_body<SCORE, VEC>(ent, rel, ph, pr, pt, n_pos, nh, nr, nt, k, cfg, loss_out, s_loss);
     cooperative_groups::this_grid().sync();
-    oct_rowopt_body<KIND>(A, B, ent.pitch, lr, blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5), gridDim.x * kWarpsPerBlock);
+    rowopt_flagged_body<KIND>(A, B, ent.pitch, lr, blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5), gridDim.x * kWarpsPerBlock);
 }
 
 // The duo scorer (oea_duo.cuh) on a fed batch: two positives per warp, octet row layout, squared-L2 score, pitch <= 128,
@@ -206,7 +206,7 @@ k_step_fed_duo(TableDev ent, TableDev rel, FedBatch F, oea_loss_cfg cfg, double*
     SampledParams none;
     duo_score_body<true>(ent, rel, none, F, cfg, loss_out, nullptr, s_loss, s_stage);
     cooperative_groups::this_grid().sync();
-    oct_rowopt_body<KIND>(A, B, ent.pitch, lr, blockIdx.x * kDuoWarps + (threadIdx.x >> 5), gridDim.x * kDuoWarps);
+    rowopt_flagged_body<KIND>(A, B, ent.pitch, lr, blockIdx.x * kDuoWarps + (threadIdx.x >> 5), gridDim.x * kDuoWarps);
 }
 
 }  // namespace oea
