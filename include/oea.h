@@ -298,6 +298,45 @@ int oea_transr_score_fed(const oea_model* model,
                          const oea_loss_cfg* loss, float loss_scale, void* workspace, size_t workspace_bytes,
                          double* loss_out, void* stream);
 
+/* ---- path (i), ProjE (models/neural/proje.py) ---------------------------------------------------------------------- */
+
+/* TF's log_uniform_candidate_sampler(unique=True, range_max) as nce_loss calls it: P(c) = log((c+2)/(c+1)) / log(E+1),
+ * draws until num_sampled distinct classes are held.  Writes the classes in draw order to sampled [num_sampled] and the
+ * number of draws taken to *num_tries (both device int32; no host synchronisation).  Draw j is a pure function of
+ * (seed, j): ⌊exp(u_j·log(E+1))⌋ − 1 mod E with u_j the top 53 bits of mix64(seed ^ mix64(j)) / 2⁵³.
+ * OEA_ERR_RANGE unless 1 <= num_sampled <= range_max; OEA_ERR_WORKSPACE when the 16-byte aligned workspace holds fewer
+ * than 4·range_max bytes (oea_proje_workspace_bytes covers it). */
+int oea_logu_sample_unique(int32_t range_max, int32_t num_sampled, uint64_t seed, int32_t* sampled, int32_t* num_tries,
+                           void* workspace, size_t workspace_bytes, void* stream);
+
+/* ProjE's variables (proje.py:36-44, :57-62).  All tables share pitch <= 128.
+ *   ent, rel  ent_embeds / rel_embeds, looked up through l2_normalize when their l2_norm is set
+ *   cls_w     entity_w [E, d], cls_b entity_b stored as [E, 1]; raw
+ *   params    [4, d]: rows mlp/mlp_w, mlp/mlp_bias, the input batch norm's beta (shared by the head and relation
+ *             inputs), the output batch norm's beta.  One table: Adam is element-wise and the four share one optimiser. */
+typedef struct oea_proje {
+    const oea_table* ent;
+    const oea_table* rel;
+    const oea_table* cls_w;
+    const oea_table* cls_b;
+    const oea_table* params;
+} oea_proje;
+
+/* ProjE's fed step, forward + backward (proje.py:46-74): x_h = ê[h], x_r = r̂[r]; both through a training-mode batch
+ * norm (batch moments, biased variance, ε = 1e-3, the shared beta); z = (y_h + y_r)∘mlp_w + mlp_bias; X = the output
+ * batch norm of z; loss = Σ_b tf.nn.nce_loss(cls_w, cls_b, label t_b, X_b) over the given sampled set (the whole batch
+ * shares it): logits x·w_c + b_c − log q(c) with q(c) = −expm1(num_tries·log1p(−P(c))), or P(c)·num_sampled when
+ * *num_tries == num_sampled; sigmoid cross-entropy, true class → 1, sampled → 0, accidental hits kept.
+ * *loss_out (device fp64) += the batch loss; every table's grad += d loss / d raw variable, touched rows flagged.
+ * FP32 throughout.  OEA_ERR_RANGE unless 1 <= num_sampled <= cls_w->rows; OEA_ERR_DIM when pitch > 128 or the pitches
+ * or dims disagree; OEA_ERR_SHAPE when cls_b is not [cls_w->rows, 1] or params not [4, dim]; OEA_ERR_WORKSPACE when the
+ * 16-byte aligned workspace is smaller than oea_proje_workspace_bytes(n_pos, num_sampled, dim, cls_w->rows).
+ * Run oea_rowopt_apply on the five tables afterwards. */
+size_t oea_proje_workspace_bytes(int32_t n_pos, int32_t num_sampled, int32_t dim, int32_t n_classes);
+int oea_proje_score_fed(const oea_proje* model, const int32_t* pos_h, const int32_t* pos_r, const int32_t* pos_t,
+                        int32_t n_pos, const int32_t* sampled, const int32_t* num_tries, int32_t num_sampled,
+                        void* workspace, size_t workspace_bytes, double* loss_out, void* stream);
+
 /* The batch producer of modules/train/batch.py:36-45 (generate_relation_triple_batch) / :168-184
  * (generate_triple_label_batch) on the device: writes the index vectors a fed step takes.
  *   pos_hrt [3, n_pos] (h | r | t rows), neg_hrt [3, n_pos·neg_per_pos] (negatives of positive p at p·k … p·k+k−1),

@@ -1,0 +1,616 @@
+// oea_proje.cu — path (i), ProjE: TF's unique log-uniform candidate sampler on the device and the step of
+// models/neural/proje.py:46-74 (a projection layer with three training-mode batch norms, then tf.nn.nce_loss over one
+// sampled set of classes the whole batch shares).  sm_90a, FP32 FFMA only.
+//
+// Maths restated from the reference and from TF 1.x (no code shared):
+//   models/neural/proje.py:51-62   x_h = ê[h], x_r = r̂[r]; y_h = BN(x_h), y_r = BN(x_r) with ONE shared beta and each its
+//                                  own batch moments; z = y_h·w + y_r·w + b (the same mlp_w twice, AUTO_REUSE); X = BN_out(z)
+//                                  BN: contrib.layers.batch_norm defaults — training mode, biased batch variance,
+//                                  ε = 1e-3, center (beta), no scale
+//   models/neural/proje.py:64-72   Σ_b nce_loss(entity_w, entity_b, t_b, X_b, num_sampled = S, num_classes = E):
+//                                  logits x·w_c + b_c − log q(c), sigmoid cross-entropy (true class → 1, sampled → 0),
+//                                  accidental hits kept
+//   LogUniformSampler              P(c) = log((c+2)/(c+1)) / log(E+1); draw = ⌊exp(u·log(E+1))⌋ − 1 mod E; unique: the
+//                                  first S distinct draws, num_tries = draws taken; expected count
+//                                  q(c) = −expm1(num_tries·log1p(−P(c))), or P(c)·S when num_tries == S (fp32, as TF)
+//
+// oea_logu_sample_unique: one CTA.  Draw j is a pure function of (seed, j).  Rounds of kRound draws: every draw
+// atomicMin's its index into first[class], so after the round's barrier draw j is new iff first[class] == j (a class
+// drawn in an earlier round, or earlier in this round, holds a smaller index).  A block scan over the new draws in draw
+// order gives their positions; the draw that takes position S − 1 writes num_tries.  Exactly the sequential loop's result.
+//
+// oea_proje_score_fed: a memset and nine kernels on `stream`, no allocation, no host synchronisation:
+//   1. k_proje_gather       one warp per positive: ê[h], r̂[r] into the workspace
+//   2. k_proje_columns_fwd  one CTA per column: both input BNs, the shared-weight combination, the output BN → X
+//   3. k_nce_logq           log q(c) of the sampled set, once
+//      k_nce_logits         128 × 128 tiles of X·W_Sᵀ (W_S = entity_w rows of the sampled set): the sampled logits'
+//                           loss, G = σ(logit) into the workspace, Σ_b G into entity_b's gradient
+//   4. k_nce_dx             dX = G·W_S, split over the sampled set so that a batch of 500 still fills the machine
+//   5. k_nce_dw             dW_S = Gᵀ·X, split over the batch, pushed with red.global.add.v4.f32 (a sampled row may also
+//                           be a label row)
+//   6. k_proje_true         one warp per positive: the true logit, its loss, g = σ(t) − 1 into dX, entity_w and entity_b
+//   7. k_proje_columns_bwd  one CTA per column: back through the three BNs and the combination; the gradients of mlp_w,
+//                           mlp_bias and both betas are this CTA's column sums
+//   8. k_proje_push         one warp per positive: dx_h, dx_r through the tables' normalisation into ent.grad, rel.grad
+#include "oea_rowmath.cuh"
+
+namespace oea {
+
+constexpr int kProjeMaxPitch = 128;
+constexpr float kBnEps = 1e-3f;                   // tf.contrib.layers.batch_norm epsilon
+constexpr int kDrawsPerThread = 16;
+constexpr int kRound = kThreads * kDrawsPerThread;
+constexpr int kTile = 128;                        // GEMM tile: 128 × 128 outputs, 16 × 16 threads of 8 × 8
+constexpr int kTk = 16;                           // reduction slice staged per iteration
+constexpr int kTld = kTile + 4;                   // shared row stride of a staged slice
+
+struct ProjeWs {
+    size_t first, xh, xr, z, x, dx, dxh, dxr, stats, lq, g, total;
+    int ldg;                                      // row stride of G: S rounded up to 4
+};
+
+// workspace sections, each 256-B aligned: the sampler's first-draw index per class, then per positive six rows of
+// `pitch` floats, eight rows of column statistics, log q of every sampled class, and G [n_pos, ldg]
+static ProjeWs proje_layout(int n_pos, int num_sampled, int pitch, int n_classes) {
+    ProjeWs w;
+    size_t at = 0;
+    auto take = [&](size_t bytes) { const size_t o = at; at += (bytes + 255) & ~(size_t)255; return o; };
+    const size_t row = 4 * (size_t)n_pos * pitch;
+    w.ldg = (num_sampled + 3) / 4 * 4;
+    w.first = take(4 * (size_t)n_classes);
+    w.xh = take(row);
+    w.xr = take(row);
+    w.z = take(row);
+    w.x = take(row);
+    w.dx = take(row);
+    w.dxh = take(row);
+    w.dxr = take(row);
+    w.stats = take(4 * 8 * (size_t)pitch);
+    w.lq = take(4 * (size_t)num_sampled);
+    w.g = take(4 * (size_t)n_pos * w.ldg);
+    w.total = at;
+    return w;
+}
+
+// ---- the sampler ---------------------------------------------------------------------------------------------------
+__host__ __device__ __forceinline__ int logu_draw(uint64_t seed, long long j, double log_range, int n_classes) {
+    const uint64_t r = mix64(seed ^ mix64((uint64_t)j));
+    const double u = (double)(r >> 11) * 0x1.0p-53;
+    const long long v = (long long)exp(u * log_range) - 1;
+    return (int)(v % n_classes);
+}
+
+// block-wide exclusive scan of one int per thread; *total gets the sum.  s has kWarpsPerBlock ints.
+__device__ __forceinline__ int block_excl_scan(int v, int* s, int* total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int u = __shfl_up_sync(OEA_FULL, inc, o);
+        if (lane >= o) inc += u;
+    }
+    if (lane == 31) s[warp] = inc;
+    __syncthreads();
+    int before = 0, all = 0;
+    for (int w = 0; w < kWarpsPerBlock; ++w) {
+        if (w < warp) before += s[w];
+        all += s[w];
+    }
+    *total = all;
+    __syncthreads();                                      // s is reused by the next scan
+    return before + inc - v;
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_logu_sample(int n_classes, int num_sampled, uint64_t seed, int32_t* __restrict__ first, int32_t* __restrict__ sampled,
+              int32_t* __restrict__ num_tries) {
+    __shared__ int s_scan[kWarpsPerBlock];
+    const double log_range = log1p((double)n_classes);
+    for (int c = threadIdx.x; c < n_classes; c += blockDim.x) first[c] = INT_MAX;
+    __syncthreads();
+    int picked = 0;                                       // block-uniform
+    for (long long base = 0; picked < num_sampled; base += kRound) {
+        int cls[kDrawsPerThread];
+        const long long j0 = base + (long long)threadIdx.x * kDrawsPerThread;
+#pragma unroll
+        for (int k = 0; k < kDrawsPerThread; ++k) {
+            cls[k] = logu_draw(seed, j0 + k, log_range, n_classes);
+            atomicMin(first + cls[k], (int)(j0 + k));
+        }
+        __syncthreads();
+        unsigned fresh = 0;
+#pragma unroll
+        for (int k = 0; k < kDrawsPerThread; ++k)
+            if (__ldcg(first + cls[k]) == (int)(j0 + k)) fresh |= 1u << k;
+        int total;
+        int at = picked + block_excl_scan(__popc(fresh), s_scan, &total);
+#pragma unroll
+        for (int k = 0; k < kDrawsPerThread; ++k) {
+            if (!((fresh >> k) & 1u)) continue;
+            if (at < num_sampled) sampled[at] = cls[k];
+            if (at == num_sampled - 1) *num_tries = (int32_t)(j0 + k + 1);
+            ++at;
+        }
+        picked += total;
+    }
+}
+
+// q(c) of TF's RangeSampler for the log-uniform distribution, in fp32
+__device__ __forceinline__ float log_expected_count(int c, int n_classes, int num_sampled, int num_tries) {
+    const float p = (float)(log((c + 2.0) / (c + 1.0)) / log1p((double)n_classes));
+    const float q = num_tries == num_sampled ? p * (float)num_sampled : -expm1f((float)num_tries * log1pf(-p));
+    return logf(q);
+}
+
+// log q(c) of every sampled class, once per call: the logits' epilogue reads it for each row tile
+__global__ void __launch_bounds__(kThreads)
+k_nce_logq(const int32_t* __restrict__ sampled, const int32_t* __restrict__ num_tries, int n_classes, int num_sampled,
+           float* __restrict__ lq) {
+    const int tries = *num_tries;
+    for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < num_sampled; s += gridDim.x * blockDim.x)
+        lq[s] = log_expected_count(__ldg(sampled + s), n_classes, num_sampled, tries);
+}
+
+__device__ __forceinline__ float sigmoid_acc(float x) { return 1.f / (1.f + expf(-x)); }
+
+struct ProjeDev {
+    TableDev ent, rel, w, b, prm;
+    int dim, pitch, n_classes, num_sampled, ldg;
+};
+
+// ---- projection layer ----------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kThreads)
+k_proje_gather(ProjeDev T, const int32_t* __restrict__ ph, const int32_t* __restrict__ pr, int n,
+               float* __restrict__ xh, float* __restrict__ xr) {
+    const int lane = threadIdx.x & 31;
+    for (int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; b < n; b += (gridDim.x * blockDim.x) >> 5) {
+        const Row<1> h = lookup<1>(T.ent, __ldg(ph + b), lane).x, r = lookup<1>(T.rel, __ldg(pr + b), lane).x;
+        if (4 * lane < T.pitch) {
+            *reinterpret_cast<float4*>(xh + (size_t)b * T.pitch + 4 * lane) = h.v[0];
+            *reinterpret_cast<float4*>(xr + (size_t)b * T.pitch + 4 * lane) = r.v[0];
+        }
+    }
+}
+
+// the sums of a and b over the block, returned to every thread
+__device__ __forceinline__ void block_sum2(float& a, float& b, float* s) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    a = warp_sum(a);
+    b = warp_sum(b);
+    if (lane == 0) { s[2 * warp] = a; s[2 * warp + 1] = b; }
+    __syncthreads();
+    a = b = 0.f;
+    for (int w = 0; w < kWarpsPerBlock; ++w) { a += s[2 * w]; b += s[2 * w + 1]; }
+    __syncthreads();
+}
+
+// stats rows: 0 μ_h, 1 rstd_h, 2 μ_r, 3 rstd_r, 4 μ_z, 5 rstd_z.  params rows: 0 mlp_w, 1 mlp_bias, 2 β_in, 3 β_out.
+__global__ void __launch_bounds__(kThreads)
+k_proje_columns_fwd(ProjeDev T, int n, const float* __restrict__ xh, const float* __restrict__ xr, float* __restrict__ z,
+                    float* __restrict__ x, float* __restrict__ stats) {
+    __shared__ float s_red[2 * kWarpsPerBlock];
+    const int P = T.pitch;
+    const float inv_n = 1.f / (float)n;
+    for (int c = blockIdx.x; c < P; c += gridDim.x) {
+        if (c >= T.dim) {                                 // padding columns of X stay zero for the head's float4 loads
+            for (int b = threadIdx.x; b < n; b += blockDim.x) x[(size_t)b * P + c] = 0.f;
+            continue;
+        }
+        float sh = 0.f, sr = 0.f;
+        for (int b = threadIdx.x; b < n; b += blockDim.x) { sh += xh[(size_t)b * P + c]; sr += xr[(size_t)b * P + c]; }
+        block_sum2(sh, sr, s_red);
+        const float mh = sh * inv_n, mr = sr * inv_n;
+        float vh = 0.f, vr = 0.f;
+        for (int b = threadIdx.x; b < n; b += blockDim.x) {
+            const float a = xh[(size_t)b * P + c] - mh, e = xr[(size_t)b * P + c] - mr;
+            vh = fmaf(a, a, vh);
+            vr = fmaf(e, e, vr);
+        }
+        block_sum2(vh, vr, s_red);
+        const float rh = rsqrtf(vh * inv_n + kBnEps), rr = rsqrtf(vr * inv_n + kBnEps);
+        const float w = T.prm.w[c], bias = T.prm.w[P + c], beta_in = T.prm.w[2 * P + c], beta_out = T.prm.w[3 * P + c];
+        float sz = 0.f, unused = 0.f;
+        for (int b = threadIdx.x; b < n; b += blockDim.x) {
+            const float yh = fmaf(xh[(size_t)b * P + c] - mh, rh, beta_in), yr = fmaf(xr[(size_t)b * P + c] - mr, rr, beta_in);
+            const float v = yh * w + yr * w + bias;
+            z[(size_t)b * P + c] = v;
+            sz += v;
+        }
+        block_sum2(sz, unused, s_red);
+        const float mz = sz * inv_n;
+        float vz = 0.f;
+        unused = 0.f;
+        for (int b = threadIdx.x; b < n; b += blockDim.x) {
+            const float a = z[(size_t)b * P + c] - mz;
+            vz = fmaf(a, a, vz);
+        }
+        block_sum2(vz, unused, s_red);
+        const float rz = rsqrtf(vz * inv_n + kBnEps);
+        for (int b = threadIdx.x; b < n; b += blockDim.x) x[(size_t)b * P + c] = fmaf(z[(size_t)b * P + c] - mz, rz, beta_out);
+        if (threadIdx.x == 0) {
+            stats[c] = mh; stats[P + c] = rh; stats[2 * P + c] = mr; stats[3 * P + c] = rr;
+            stats[4 * P + c] = mz; stats[5 * P + c] = rz;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_proje_columns_bwd(ProjeDev T, int n, const float* __restrict__ xh, const float* __restrict__ xr,
+                    const float* __restrict__ z, float* __restrict__ dx, const float* __restrict__ stats,
+                    float* __restrict__ dxh, float* __restrict__ dxr) {
+    __shared__ float s_red[2 * kWarpsPerBlock];
+    const int P = T.pitch;
+    const float inv_n = 1.f / (float)n;
+    for (int c = blockIdx.x; c < P; c += gridDim.x) {
+        if (c >= T.dim) {                                 // padding columns: the push reads whole rows
+            for (int b = threadIdx.x; b < n; b += blockDim.x) dxh[(size_t)b * P + c] = dxr[(size_t)b * P + c] = 0.f;
+            continue;
+        }
+        const float mh = stats[c], rh = stats[P + c], mr = stats[2 * P + c], rr = stats[3 * P + c];
+        const float mz = stats[4 * P + c], rz = stats[5 * P + c];
+        const float w = T.prm.w[c], beta_in = T.prm.w[2 * P + c];
+        // output BN: dβ_out = Σ dX, dz = rstd·(dX − mean dX − ẑ·mean(dX·ẑ))
+        float s1 = 0.f, s2 = 0.f;
+        for (int b = threadIdx.x; b < n; b += blockDim.x) {
+            const float g = dx[(size_t)b * P + c];
+            s1 += g;
+            s2 = fmaf(g, (z[(size_t)b * P + c] - mz) * rz, s2);
+        }
+        block_sum2(s1, s2, s_red);
+        const float m1 = s1 * inv_n, m2 = s2 * inv_n;
+        // dz (stored over dX), and the sums the combination and the input BNs need
+        float sdz = 0.f, sdw = 0.f, sh = 0.f, sr = 0.f;
+        for (int b = threadIdx.x; b < n; b += blockDim.x) {
+            const size_t i = (size_t)b * P + c;
+            const float zh = (z[i] - mz) * rz;
+            const float dz = rz * (dx[i] - m1 - zh * m2);
+            dx[i] = dz;
+            const float nh = (xh[i] - mh) * rh, nr = (xr[i] - mr) * rr;
+            sdz += dz;
+            sdw = fmaf(dz, nh + beta_in + nr + beta_in, sdw);
+            sh = fmaf(dz, nh, sh);
+            sr = fmaf(dz, nr, sr);
+        }
+        block_sum2(sdz, sdw, s_red);
+        block_sum2(sh, sr, s_red);
+        // input BNs: dy = w·dz for both; dx̂ = rstd·(dy − mean dy − x̂·mean(dy·x̂))
+        const float md = w * sdz * inv_n, mdh = w * sh * inv_n, mdr = w * sr * inv_n;
+        for (int b = threadIdx.x; b < n; b += blockDim.x) {
+            const size_t i = (size_t)b * P + c;
+            const float dy = w * dx[i];
+            dxh[i] = rh * (dy - md - (xh[i] - mh) * rh * mdh);
+            dxr[i] = rr * (dy - md - (xr[i] - mr) * rr * mdr);
+        }
+        if (threadIdx.x == 0) {
+            T.prm.g[c] += sdw;
+            T.prm.g[P + c] += sdz;
+            T.prm.g[2 * P + c] += 2.f * w * sdz;
+            T.prm.g[3 * P + c] += s1;
+            if (c == 0)
+                for (int r = 0; r < 4; ++r) T.prm.touched[r] = 1;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_proje_push(ProjeDev T, const int32_t* __restrict__ ph, const int32_t* __restrict__ pr, int n,
+             const float* __restrict__ dxh, const float* __restrict__ dxr) {
+    const int lane = threadIdx.x & 31;
+    for (int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; b < n; b += (gridDim.x * blockDim.x) >> 5) {
+        const int h = __ldg(ph + b), r = __ldg(pr + b);
+        push<1>(T.ent, h, lane, load_row<1>(dxh, b, T.pitch, lane), lookup<1>(T.ent, h, lane));
+        push<1>(T.rel, r, lane, load_row<1>(dxr, b, T.pitch, lane), lookup<1>(T.rel, r, lane));
+    }
+}
+
+// ---- the NCE head: 128 × 128 FP32 register tiles -------------------------------------------------------------------
+// C[m][n] += Σ_{k<kTk} As[k][m]·Bs[k][n] for this thread's 8 × 8 outputs m = ty + 16a, n = tx + 16b.  The 16 threads of
+// a half-warp share ty (one broadcast address of As) and read 16 consecutive n of Bs: conflict-free.
+__device__ __forceinline__ void tile_mma(float (&acc)[8][8], const float* As, const float* Bs, int ty, int tx) {
+#pragma unroll
+    for (int k = 0; k < kTk; ++k) {
+        float av[8], bv[8];
+#pragma unroll
+        for (int a = 0; a < 8; ++a) av[a] = As[k * kTld + ty + 16 * a];
+#pragma unroll
+        for (int b = 0; b < 8; ++b) bv[b] = Bs[k * kTld + tx + 16 * b];
+#pragma unroll
+        for (int a = 0; a < 8; ++a)
+#pragma unroll
+            for (int b = 0; b < 8; ++b) acc[a][b] = fmaf(av[a], bv[b], acc[a][b]);
+    }
+}
+
+// S[k][i] = src(row i, column k0 + k) for i < 128, k < kTk, from rows contiguous along k (row pointer rp(i), or nullptr
+// for a row outside the operand); columns at or past kn read as 0.  kn and k0 are multiples of 4.
+template <class RowPtr>
+__device__ __forceinline__ void stage_rows_t(float* S, RowPtr rp, int k0, int kn) {
+    for (int e = threadIdx.x; e < kTile * (kTk / 4); e += blockDim.x) {
+        const int i = e >> 2, q = e & 3, k = k0 + 4 * q;
+        const float* p = rp(i);
+        const float4 v = (p != nullptr && k < kn) ? ldg4(p + k) : f4(0.f);
+        S[(4 * q) * kTld + i] = v.x; S[(4 * q + 1) * kTld + i] = v.y;
+        S[(4 * q + 2) * kTld + i] = v.z; S[(4 * q + 3) * kTld + i] = v.w;
+    }
+}
+
+// S[k][i] = src(row k, column i) for k < kTk, i < 128, from rows contiguous along i (row pointer rp(k), or nullptr);
+// columns at or past cn read as 0.  cn is a multiple of 4.
+template <class RowPtr>
+__device__ __forceinline__ void stage_rows_n(float* S, RowPtr rp, int cn) {
+    for (int e = threadIdx.x; e < kTk * (kTile / 4); e += blockDim.x) {
+        const int k = e >> 5, i = 4 * (e & 31);
+        const float* p = rp(k);
+        const float4 v = (p != nullptr && i < cn) ? ldg4(p + i) : f4(0.f);
+        *reinterpret_cast<float4*>(S + k * kTld + i) = v;
+    }
+}
+
+__device__ __forceinline__ void zero_acc(float (&acc)[8][8]) {
+#pragma unroll
+    for (int a = 0; a < 8; ++a)
+#pragma unroll
+        for (int b = 0; b < 8; ++b) acc[a][b] = 0.f;
+}
+
+// logits of the sampled classes: tile (bt, st) of [n × S]; G = σ(logit) for the backward, Σ_b G into entity_b's gradient
+__global__ void __launch_bounds__(kThreads)
+k_nce_logits(ProjeDev T, int n, const float* __restrict__ x, const int32_t* __restrict__ sampled,
+             const float* __restrict__ lqs, float* __restrict__ G, double* __restrict__ loss_out) {
+    __shared__ __align__(16) float As[kTk * kTld];
+    __shared__ __align__(16) float Bs[kTk * kTld];
+    __shared__ float s_db[kTile];
+    __shared__ double s_loss[kWarpsPerBlock];
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    const int S = T.num_sampled;
+    const int mt = (n + kTile - 1) / kTile, nt = (T.ldg + kTile - 1) / kTile;
+    float lsum = 0.f;
+    for (int t = blockIdx.x; t < mt * nt; t += gridDim.x) {
+        const int m0 = (t % mt) * kTile, n0 = (t / mt) * kTile;
+        float acc[8][8];
+        zero_acc(acc);
+        for (int k0 = 0; k0 < T.pitch; k0 += kTk) {
+            __syncthreads();
+            stage_rows_t(As, [&](int i) { return m0 + i < n ? x + (size_t)(m0 + i) * T.pitch : nullptr; }, k0, T.pitch);
+            stage_rows_t(Bs, [&](int i) { return n0 + i < S ? T.w.w + (size_t)__ldg(sampled + n0 + i) * T.pitch : nullptr; },
+                         k0, T.pitch);
+            __syncthreads();
+            tile_mma(acc, As, Bs, ty, tx);
+        }
+        if (threadIdx.x < kTile) s_db[threadIdx.x] = 0.f;
+        __syncthreads();
+#pragma unroll
+        for (int b = 0; b < 8; ++b) {
+            const int s = n0 + tx + 16 * b;
+            float bias = 0.f, lq = 0.f;
+            if (s < S) {
+                const int c = __ldg(sampled + s);
+                bias = T.b.w[(size_t)c * T.b.pitch];
+                lq = __ldg(lqs + s);
+            }
+            float col = 0.f;
+#pragma unroll
+            for (int a = 0; a < 8; ++a) {
+                const int m = m0 + ty + 16 * a;
+                if (m >= n || s >= T.ldg) continue;
+                float g = 0.f;
+                if (s < S) {
+                    const float logit = acc[a][b] + bias - lq;
+                    lsum += softplus(logit);
+                    g = sigmoid_acc(logit);
+                    col += g;
+                }
+                G[(size_t)m * T.ldg + s] = g;
+            }
+            if (s < S) atomicAdd(s_db + tx + 16 * b, col);
+        }
+        __syncthreads();
+        if (threadIdx.x < kTile && n0 + (int)threadIdx.x < S) {
+            const int c = __ldg(sampled + n0 + threadIdx.x);
+            atomicAdd(T.b.g + (size_t)c * T.b.pitch, s_db[threadIdx.x]);
+            if (m0 == 0) { T.b.touched[c] = 1; T.w.touched[c] = 1; }
+        }
+    }
+    LossAcc lacc{s_loss};
+    lacc.flush(warp_sum(lsum), loss_out);
+}
+
+// dX[b][:] += Σ_{s in split} G[b][s]·W_S[s][:]; tile t = (b tile, split of the sampled set)
+__global__ void __launch_bounds__(kThreads)
+k_nce_dx(ProjeDev T, int n, const float* __restrict__ G, const int32_t* __restrict__ sampled, int split,
+         float* __restrict__ dx) {
+    __shared__ __align__(16) float As[kTk * kTld];
+    __shared__ __align__(16) float Bs[kTk * kTld];
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    const int S = T.num_sampled;
+    const int mt = (n + kTile - 1) / kTile, st = (S + split - 1) / split;
+    for (int t = blockIdx.x; t < mt * st; t += gridDim.x) {
+        const int m0 = (t % mt) * kTile, s0 = (t / mt) * split, s1 = min(S, s0 + split);
+        float acc[8][8];
+        zero_acc(acc);
+        for (int k0 = s0; k0 < s1; k0 += kTk) {
+            __syncthreads();
+            // A(b, s) = G[b][s]: rows along s.  A split ends on a multiple of kTk or at S, and G's columns S … ldg − 1
+            // are zero, so the slice needs no clipping inside a float4
+            stage_rows_t(As, [&](int i) { return m0 + i < n ? G + (size_t)(m0 + i) * T.ldg : nullptr; }, k0,
+                         (s1 + 3) / 4 * 4);
+            stage_rows_n(Bs, [&](int k) { return k0 + k < s1 ? T.w.w + (size_t)__ldg(sampled + k0 + k) * T.pitch : nullptr; },
+                         T.pitch);
+            __syncthreads();
+            tile_mma(acc, As, Bs, ty, tx);
+        }
+#pragma unroll
+        for (int a = 0; a < 8; ++a) {
+            const int m = m0 + ty + 16 * a;
+            if (m >= n) continue;
+#pragma unroll
+            for (int b = 0; b < 8; ++b) {
+                const int c = tx + 16 * b;
+                if (c < T.dim) atomicAdd(dx + (size_t)m * T.pitch + c, acc[a][b]);
+            }
+        }
+    }
+}
+
+// entity_w.grad[sampled[s]][:] += Σ_{b in split} G[b][s]·X[b][:]; tile t = (sampled tile, split of the batch)
+__global__ void __launch_bounds__(kThreads)
+k_nce_dw(ProjeDev T, int n, const float* __restrict__ G, const float* __restrict__ x, const int32_t* __restrict__ sampled,
+         int split) {
+    __shared__ __align__(16) float As[kTk * kTld];
+    __shared__ __align__(16) float Bs[kTk * kTld];
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    const int S = T.num_sampled;
+    const int mt = (S + kTile - 1) / kTile, bt = (n + split - 1) / split;
+    for (int t = blockIdx.x; t < mt * bt; t += gridDim.x) {
+        const int m0 = (t % mt) * kTile, b0 = (t / mt) * split, b1 = min(n, b0 + split);
+        float acc[8][8];
+        zero_acc(acc);
+        for (int k0 = b0; k0 < b1; k0 += kTk) {
+            __syncthreads();
+            // A(s, b) = G[b][s]: G's rows run along s, so the slice is staged without a transpose
+            stage_rows_n(As, [&](int k) { return k0 + k < b1 ? G + (size_t)(k0 + k) * T.ldg + m0 : nullptr; },
+                         min(kTile, T.ldg - m0));
+            stage_rows_n(Bs, [&](int k) { return k0 + k < b1 ? x + (size_t)(k0 + k) * T.pitch : nullptr; }, T.pitch);
+            __syncthreads();
+            tile_mma(acc, As, Bs, ty, tx);
+        }
+        // rows of 128 floats in registers are 8 strided columns per thread: go through shared memory for float4 reds
+        __syncthreads();
+        float* Cs = As;                                   // 16 rows at a time
+#pragma unroll
+        for (int a = 0; a < 8; ++a) {
+#pragma unroll
+            for (int b = 0; b < 8; ++b) Cs[ty * kTld + tx + 16 * b] = acc[a][b];
+            __syncthreads();
+            for (int e = threadIdx.x; e < 16 * (kTile / 4); e += blockDim.x) {
+                const int r = e >> 5, c = 4 * (e & 31), s = m0 + r + 16 * a;
+                if (s < S && c < T.pitch)
+                    red_add4(T.w.g + (size_t)__ldg(sampled + s) * T.pitch + c,
+                             *reinterpret_cast<const float4*>(Cs + r * kTld + c));
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// the true class of every positive: logit, loss, and its whole backward (dX row, entity_w and entity_b rows)
+__global__ void __launch_bounds__(kThreads)
+k_proje_true(ProjeDev T, const int32_t* __restrict__ pt, int n, const float* __restrict__ x,
+             const int32_t* __restrict__ num_tries, float* __restrict__ dx, double* __restrict__ loss_out) {
+    __shared__ double s_loss[kWarpsPerBlock];
+    const int lane = threadIdx.x & 31;
+    const int tries = *num_tries;
+    float lsum = 0.f;
+    for (int b0 = (blockIdx.x * blockDim.x) >> 5; b0 < n; b0 += (gridDim.x * blockDim.x) >> 5) {   // warp-uniform
+        const int b = b0 + (threadIdx.x >> 5);
+        if (b >= n) continue;
+        const int c = __ldg(pt + b);
+        const Row<1> xb = load_row<1>(x, b, T.pitch, lane), wc = load_row<1>(T.w.w, c, T.pitch, lane);
+        const float logit = warp_sum(dotr(xb, wc)) + T.b.w[(size_t)c * T.b.pitch] -
+                            log_expected_count(c, T.n_classes, T.num_sampled, tries);
+        const float g = -sigmoid_acc(-logit);             // σ(t) − 1
+        if (lane == 0) {
+            lsum += softplus(-logit);
+            atomicAdd(T.b.g + (size_t)c * T.b.pitch, g);
+            T.b.touched[c] = 1;
+            T.w.touched[c] = 1;
+        }
+        if (4 * lane < T.pitch) {
+            float4* d = reinterpret_cast<float4*>(dx + (size_t)b * T.pitch + 4 * lane);
+            *d = fma4(wc.v[0], g, *d);
+        }
+        red_row<1>(T.w.g, c, T.pitch, lane, r_scale(xb, g));
+    }
+    LossAcc lacc{s_loss};
+    lacc.flush(warp_sum(lsum), loss_out);
+}
+
+}  // namespace oea
+
+using namespace oea;
+
+extern "C" size_t oea_proje_workspace_bytes(int32_t n_pos, int32_t num_sampled, int32_t dim, int32_t n_classes) {
+    if (n_pos < 0 || num_sampled < 1 || dim <= 0 || n_classes <= 0) return 0;
+    return proje_layout(n_pos, num_sampled, (dim + 3) / 4 * 4, n_classes).total;
+}
+
+extern "C" int oea_logu_sample_unique(int32_t range_max, int32_t num_sampled, uint64_t seed, int32_t* sampled,
+                                      int32_t* num_tries, void* workspace, size_t workspace_bytes, void* stream) {
+    if (range_max < 1 || num_sampled < 1 || num_sampled > range_max) return OEA_ERR_RANGE;
+    if (sampled == nullptr || num_tries == nullptr) return OEA_ERR_NULL;
+    if (workspace == nullptr || workspace_bytes < 4 * (size_t)range_max || !aligned16(workspace)) return OEA_ERR_WORKSPACE;
+    OEA_LAUNCH(k_logu_sample, 1, kThreads, 0, (cudaStream_t)stream, range_max, num_sampled, seed,
+               static_cast<int32_t*>(workspace), sampled, num_tries);
+    OEA_LAUNCH_CHECK();
+    return OEA_OK;
+}
+
+extern "C" int oea_proje_score_fed(const oea_proje* model, const int32_t* pos_h, const int32_t* pos_r,
+                                   const int32_t* pos_t, int32_t n_pos, const int32_t* sampled, const int32_t* num_tries,
+                                   int32_t num_sampled, void* workspace, size_t workspace_bytes, double* loss_out,
+                                   void* stream) {
+    if (model == nullptr) return OEA_ERR_NULL;
+    const oea_table* tabs[5] = {model->ent, model->rel, model->cls_w, model->cls_b, model->params};
+    for (const oea_table* t : tabs) {
+        const int rc = check_table(t, true);
+        if (rc) return rc;
+    }
+    const oea_table *ent = model->ent, *rel = model->rel, *w = model->cls_w, *b = model->cls_b, *prm = model->params;
+    if (rel->dim != ent->dim || w->dim != ent->dim || rel->pitch != ent->pitch || w->pitch != ent->pitch ||
+        prm->pitch != ent->pitch || ent->pitch > kProjeMaxPitch)
+        return OEA_ERR_DIM;
+    if (b->rows != w->rows || b->dim != 1 || prm->rows != 4 || prm->dim != ent->dim) return OEA_ERR_SHAPE;
+    if (num_sampled < 1 || num_sampled > w->rows) return OEA_ERR_RANGE;
+    if (n_pos < 0) return OEA_ERR_SHAPE;
+    if (sampled == nullptr || num_tries == nullptr || loss_out == nullptr) return OEA_ERR_NULL;
+    if (n_pos > 0 && (!pos_h || !pos_r || !pos_t)) return OEA_ERR_NULL;
+    const ProjeWs L = proje_layout(n_pos, num_sampled, ent->pitch, w->rows);
+    if (workspace == nullptr || workspace_bytes < L.total || !aligned16(workspace)) return OEA_ERR_WORKSPACE;
+    if (n_pos == 0) return OEA_OK;
+
+    char* ws = static_cast<char*>(workspace);
+    float* xh = reinterpret_cast<float*>(ws + L.xh);
+    float* xr = reinterpret_cast<float*>(ws + L.xr);
+    float* z = reinterpret_cast<float*>(ws + L.z);
+    float* x = reinterpret_cast<float*>(ws + L.x);
+    float* dx = reinterpret_cast<float*>(ws + L.dx);
+    float* dxh = reinterpret_cast<float*>(ws + L.dxh);
+    float* dxr = reinterpret_cast<float*>(ws + L.dxr);
+    float* stats = reinterpret_cast<float*>(ws + L.stats);
+    float* lq = reinterpret_cast<float*>(ws + L.lq);
+    float* G = reinterpret_cast<float*>(ws + L.g);
+    ProjeDev T;
+    T.ent = table_dev(ent); T.rel = table_dev(rel); T.w = table_dev(w); T.b = table_dev(b); T.prm = table_dev(prm);
+    T.w.norm = T.b.norm = T.prm.norm = false;             // entity_w, entity_b and the MLP / BN variables: raw
+    T.dim = ent->dim; T.pitch = ent->pitch; T.n_classes = w->rows; T.num_sampled = num_sampled; T.ldg = L.ldg;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int n = n_pos, S = num_sampled;
+#ifdef OEA_HOST_EMU   // tests/emu: grid-stride kernels on two blocks keep the emulated thread count small
+    const int rows_grid = 2, col_grid = 2, lg_grid = 2, dx_grid = 2, dw_grid = 2;
+    const int split_s = 2 * kTk, split_b = 2 * kTk;       // several splits even on small cases
+#else
+    const int mt_b = (n + kTile - 1) / kTile, mt_s = (S + kTile - 1) / kTile;
+    const int rows_grid = grid_for(n);
+    const int col_grid = ent->pitch;
+    const int lg_grid = mt_b * ((L.ldg + kTile - 1) / kTile);
+    // split each reduction so that about two CTAs per SM run: a batch of 500 is only four row tiles, and S = 4096
+    // only 32 column tiles.  A split is a multiple of kTk.
+    const int want = 2 * sm_count_cached();
+    auto split_of = [](int len, int parts) { const int s = (len + parts - 1) / parts; return (s + kTk - 1) / kTk * kTk; };
+    const int split_s = split_of(S, (want + mt_b - 1) / mt_b), split_b = split_of(n, (want + mt_s - 1) / mt_s);
+    const int dx_grid = mt_b * ((S + split_s - 1) / split_s);
+    const int dw_grid = mt_s * ((n + split_b - 1) / split_b);
+#endif
+    OEA_CUDA_TRY(cudaMemsetAsync(dx, 0, 4 * (size_t)n * ent->pitch, st));
+    OEA_LAUNCH(k_proje_gather, rows_grid, kThreads, 0, st, T, pos_h, pos_r, n, xh, xr);
+    OEA_LAUNCH(k_proje_columns_fwd, col_grid, kThreads, 0, st, T, n, xh, xr, z, x, stats);
+    OEA_LAUNCH(k_nce_logq, rows_grid, kThreads, 0, st, sampled, num_tries, T.n_classes, S, lq);
+    OEA_LAUNCH(k_nce_logits, lg_grid, kThreads, 0, st, T, n, x, sampled, lq, G, loss_out);
+    OEA_LAUNCH(k_nce_dx, dx_grid, kThreads, 0, st, T, n, G, sampled, split_s, dx);
+    OEA_LAUNCH(k_nce_dw, dw_grid, kThreads, 0, st, T, n, G, x, sampled, split_b);
+    OEA_LAUNCH(k_proje_true, rows_grid, kThreads, 0, st, T, pos_t, n, x, num_tries, dx, loss_out);
+    OEA_LAUNCH(k_proje_columns_bwd, col_grid, kThreads, 0, st, T, n, xh, xr, z, dx, stats, dxh, dxr);
+    OEA_LAUNCH(k_proje_push, rows_grid, kThreads, 0, st, T, pos_h, pos_r, n, dxh, dxr);
+    OEA_LAUNCH_CHECK();
+    return OEA_OK;
+}

@@ -497,6 +497,99 @@ class ModelTrainer:
         return v
 
 
+class ProjETrainer:
+    """ProjE's step (models/neural/proje.py:46-96): device batch producer (oea_triple_sample_batch, positives only) →
+    TF's unique log-uniform sampler on the device (oea_logu_sample_unique; one set of `num_sampled` classes per step,
+    seeded from the epoch seed and the step) → the projection layer and the NCE head (oea_proje_score_fed) → Adam on the
+    five tables.  tables = (ent, rel, cls_w, cls_b, params) EmbeddingTables: entity_w, entity_b as [E, 1], and the
+    [4, d] table of mlp_w, mlp_bias and the two batch-norm betas.  The workspace grows on demand."""
+
+    def __init__(self, tables, num_sampled, lr, sampler="fast"):
+        self.lib = L.load()
+        self.tables = tuple(tables)
+        self.num_sampled = int(num_sampled)
+        n_classes = self.tables[2].rows
+        if not 1 <= self.num_sampled <= n_classes:
+            raise ValueError("nce_loss samples %d distinct classes out of %d: the sampler's range is too small"
+                             % (self.num_sampled, n_classes))
+        self.lr = float(lr)
+        self.sampler = {"fast": 0, "independent": 1}[sampler]
+        dev = self.tables[0].device
+        self.loss_dev = torch.zeros(1, dtype=torch.float64, device=dev)
+        self.sampled = torch.zeros(self.num_sampled, dtype=torch.int32, device=dev)
+        self.num_tries = torch.zeros(1, dtype=torch.int32, device=dev)
+        self._idx = None
+        self._n_pos = C.c_int32(0)
+        self._ws = None
+
+    def _workspace(self, n_pos):
+        need = self.lib.oea_proje_workspace_bytes(n_pos, self.num_sampled, self.tables[0].dim, self.tables[2].rows)
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(max(1, need), dtype=torch.uint8, device=self.tables[0].device)
+        return self._ws
+
+    def _c_model(self):
+        return L.Proje(*[C.pointer(t.c_struct()) for t in self.tables])
+
+    def sample(self, seed):
+        """Draw the step's sampled set into self.sampled / self.num_tries (device; no host synchronisation)."""
+        ws = self._workspace(0)
+        L.check(self.lib.oea_logu_sample_unique(self.tables[2].rows, self.num_sampled, int(seed) & (2**64 - 1),
+                                                _ptr(self.sampled), _ptr(self.num_tries), _ptr(ws), ws.numel(),
+                                                _stream_ptr()), "oea_logu_sample_unique")
+
+    def score_fed(self, pos, sampled=None, num_tries=None, loss_out=None):
+        """pos: int32 device tensor [3, n] (h | r | t rows); sampled / num_tries: int32 device tensors (default: the
+        last sample()).  Accumulates gradients into the five tables and adds the batch loss into loss_out."""
+        out = self.loss_dev if loss_out is None else loss_out
+        sampled = self.sampled if sampled is None else sampled
+        num_tries = self.num_tries if num_tries is None else num_tries
+        n_pos = pos.shape[1]
+        ws = self._workspace(n_pos)
+        model = self._c_model()
+        np_ = lambda i: C.c_void_p(0 if n_pos == 0 else pos[i].data_ptr())
+        L.check(self.lib.oea_proje_score_fed(C.byref(model), np_(0), np_(1), np_(2), n_pos, _ptr(sampled),
+                                             _ptr(num_tries), sampled.numel(), _ptr(ws), ws.numel(), _ptr(out),
+                                             _stream_ptr()), "oea_proje_score_fed")
+
+    def apply(self):
+        for tab in self.tables:
+            tab.apply(self.lr)
+
+    def sample_batch(self, kg1, kg2, tset, batch_size, step, epoch_seed, max_try=10):
+        """The device batch producer with no negatives: pos [3, n_pos] int32 device tensor."""
+        if self._idx is None or self._idx.numel() < 3 * batch_size:
+            self._idx = torch.empty(3 * batch_size, dtype=torch.int32, device=self.tables[0].device)
+        smp = L.SampleCfg(int(batch_size), 0, int(step), int(max_try), int(epoch_seed) & (2**64 - 1), 0)
+        k1, k2, ts = kg1.view(), kg2.view(), tset.view()
+        L.check(self.lib.oea_triple_sample_batch(
+            C.byref(k1), C.byref(k2), C.byref(ts), C.byref(smp), self.sampler, C.byref(self.tables[0].c_struct()),
+            _ptr(self._idx), C.c_void_p(0), C.byref(self._n_pos), _stream_ptr()), "oea_triple_sample_batch")
+        n = int(self._n_pos.value)
+        return self._idx[:3 * n].view(3, n)
+
+    @staticmethod
+    def step_seed(epoch_seed, step):
+        """The sampler's seed of one step: a function of (epoch seed, step) only, so that a resumed run draws the same."""
+        return (int(epoch_seed) * 0x9E3779B97F4A7C15 + int(step) + 1) & (2**64 - 1)
+
+    def step_sampled(self, kg1, kg2, tset, batch_size, neg_per_pos, step, epoch_seed, max_try=10, **_):
+        """One session.run([triple_loss, triple_optimizer]) of proje.py:87-90; neg_per_pos is ignored (positives only)."""
+        pos = self.sample_batch(kg1, kg2, tset, batch_size, step, epoch_seed, max_try)
+        if pos.shape[1] == 0:
+            return 0
+        self.sample(self.step_seed(epoch_seed, step))
+        self.score_fed(pos)
+        self.apply()
+        return pos.shape[1]
+
+    def read_loss(self, reset=True):
+        v = float(self.loss_dev.item())
+        if reset:
+            self.loss_dev.zero_()
+        return v
+
+
 class FedHostPipeline:
     """Depth-2 pipeline over TripleTrainer's host-index step (oea_triple_step_fed_host_submit / _collect): the copy of
     step i+1 overlaps the kernels of step i; losses come back one step late.  Owns two streams, four events and the

@@ -86,6 +86,11 @@ class SeedXchg(C.Structure):
                 ("ticket", C.c_void_p)]
 
 
+class Proje(C.Structure):
+    # oea_proje: ent_embeds, rel_embeds, entity_w, entity_b ([E, 1]) and the [4, d] table of mlp_w, mlp_bias and the betas
+    _fields_ = [("ent", _TP), ("rel", _TP), ("cls_w", _TP), ("cls_b", _TP), ("params", _TP)]
+
+
 class Model(C.Structure):
     # gamma / phase: RotatE's model constants (0 and ignored for the other kinds)
     _fields_ = [("kind", C.c_int32), ("ent", _TP), ("rel", _TP), ("ent_aux", _TP), ("rel_aux", _TP),
@@ -149,6 +154,9 @@ SIGNATURES = {
     "oea_transr_workspace_bytes": (C.c_size_t, [_I, _I, _I, _I]),
     "oea_transr_score_fed": (C.c_int, [C.POINTER(Model), _P, _P, _P, _I, _P, _P, _P, _I, C.POINTER(LossCfg), C.c_float,
                                        _P, C.c_size_t, _P, _P]),
+    "oea_logu_sample_unique": (C.c_int, [_I, _I, C.c_uint64, _P, _P, _P, C.c_size_t, _P]),
+    "oea_proje_workspace_bytes": (C.c_size_t, [_I, _I, _I, _I]),
+    "oea_proje_score_fed": (C.c_int, [C.POINTER(Proje), _P, _P, _P, _I, _P, _P, _I, _P, C.c_size_t, _P, _P]),
     "oea_rows_gather_sort": (C.c_int, [_P, _L, _I, _I, _P, _P, _P]),
     "oea_gale_shapley_workspace_bytes": (C.c_size_t, [_I, _I]),
     "oea_gale_shapley": (C.c_int, [_P, _P, _I, _I, _I, _I, _P, _P, C.c_size_t, C.POINTER(C.c_int32), _P]),

@@ -422,7 +422,9 @@ class BasicModel:
         steps_tasks = task_divide(list(range(triple_steps)), self.args.batch_threads_num)
         neighbors1, neighbors2 = None, None
         start_epoch = getattr(self, "_start_epoch", 1)
-        if start_epoch > 1 and self.args.neg_sampling == 'truncated' and (start_epoch - 1) >= self.args.truncated_freq:
+        # ProjE's configuration names no neg_sampling (its batches are positives only)
+        truncated = getattr(self.args, "neg_sampling", None) == 'truncated'
+        if start_epoch > 1 and truncated and (start_epoch - 1) >= self.args.truncated_freq:
             neighbors1, neighbors2 = self._refresh_neighbours()     # the candidate lists are derived state: rebuild them
         every = getattr(self.args, "checkpoint_every", 0)
         for i in range(start_epoch, self.args.max_epoch + 1):
@@ -435,7 +437,7 @@ class BasicModel:
                 self.flag1, self.flag2, self.early_stop = early_stop(self.flag1, self.flag2, flag)
                 if self.early_stop or i == self.args.max_epoch:
                     break
-            if self.args.neg_sampling == 'truncated' and i % self.args.truncated_freq == 0:
+            if truncated and i % self.args.truncated_freq == 0:
                 t1 = time.time()
                 neighbors1 = neighbors2 = None
                 gc.collect()

@@ -61,8 +61,10 @@ def init_values(shape, init):
 
 
 def _xavier_values(shape):
-    # tf.contrib.layers.xavier_initializer(uniform=False): truncated normal, σ = sqrt(1.3·2/(fan_in+fan_out))
-    return _trunc_normal(shape, math.sqrt(1.3 * 2.0 / (shape[0] + shape[1])))
+    # tf.contrib.layers.xavier_initializer(uniform=False): truncated normal, σ = sqrt(1.3·2/(fan_in+fan_out)); a 1-D
+    # shape [n] has fan_in = fan_out = n (ProjE's entity_b), so σ = sqrt(1.3/n)
+    fan_in, fan_out = (shape[0], shape[1]) if len(shape) > 1 else (shape[0], shape[0])
+    return _trunc_normal(shape, math.sqrt(1.3 * 2.0 / (fan_in + fan_out)))
 
 
 def _normal_values(shape):

@@ -87,6 +87,15 @@ def transr(scale="15K"):
                  test_threads_num=4, eval_metric="inner", eval_norm=False)
 
 
+def proje(scale="15K"):
+    """run/args/proje_args_15K.json and proje_args_100K.json."""
+    small = scale == "15K"
+    return _args(embedding_module="ProjE", alignment_module="sharing", dim=100, init="xavier", ent_l2_norm=True,
+                 rel_l2_norm=True, learning_rate=0.001, optimizer="Adam", batch_size=500 if small else 5000,
+                 dnn_neg_nums=4096, batch_threads_num=2 if small else 3, test_threads_num=2 if small else 10,
+                 start_valid=100 if small else 300, eval_metric="inner", eval_norm=True)
+
+
 def simple(scale="15K"):
     return _args(embedding_module="SimplE", alignment_module="sharing", dim=100, init="xavier", ent_l2_norm=True,
                  rel_l2_norm=True, learning_rate=0.01, optimizer="Adagrad", batch_size=5000 if scale == "15K" else 20000,
