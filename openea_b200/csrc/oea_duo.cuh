@@ -19,6 +19,7 @@
 #include "oea_rowmath.cuh"
 #include "oea_rowopt.cuh"
 #include "oea_sampler.cuh"
+#include "oea_transe.cuh"
 
 namespace oea {
 
@@ -72,13 +73,6 @@ struct DuoStage {
     float4 rt[2][4][8];
     float4 Eh[4][32];
     float4 Et[4][32];
-};
-
-// index vectors of a fed batch (device pointers)
-struct FedBatch {
-    const int32_t* ph; const int32_t* pr; const int32_t* pt;
-    const int32_t* nh; const int32_t* nr; const int32_t* nt;
-    int n_pos, k;
 };
 
 // Negative sampling of TWO positives by one warp: warp_sample_negatives (oea_sampler.cuh) with lane (half, hl) owning

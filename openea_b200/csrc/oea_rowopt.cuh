@@ -15,7 +15,7 @@ struct OptTab {
 };
 
 // Row optimiser over [A rows | B rows] (same pitch), flagged rows only; TF1 Adagrad (acc += g², x −= lr·g/√acc) or
-// SGD as in k_rowopt, then g = 0 and the flag cleared.  Padding columns are left as they are.
+// SGD (x −= lr·g), then g = 0 and the flag cleared.  Padding columns are left as they are.
 //
 // The work unit is a quad of 4 consecutive rows.  Warp w owns quads w, w + n_warps, … : strided, because entity ids
 // are ordered by degree and the flagged rows cluster at low ids.  It walks them in windows of 32 quads, lane j taking

@@ -1,5 +1,5 @@
-// oea_triple.cu — path (i): negative-sampled triple scoring forward+backward (K1), the row
-// optimiser, the fused on-device sampler, and the table lookup.  sm_90a.
+// oea_triple.cu — path (i): the sampled scorers and steps (K1: negative-sampled triple scoring forward+backward
+// with the fused on-device sampler), the row optimiser, and the table lookup.  sm_90a.
 //
 // Maths restated from the reference (no code shared):
 //   modules/base/losses.py:15-73      score + losses (sums, squared L2)
@@ -8,142 +8,18 @@
 //   modules/train/batch.py:36-119     batch slicing + corrupt-head/tail negative sampling
 //   approaches/bootea.py:197          alignment loss
 //
-// Work decomposition: one warp per triple (fed path) or per positive + its k negatives (sampled
-// path).  A row of `dim` floats is held as VEC float4 per lane (dim <= 128·VEC), loaded with
-// 128-bit coalesced reads; row reductions are warp shuffles; gradients leave through 128-bit
-// vector reductions (red.global.add.v4.f32) into the L2-resident gradient table.
+// Work decomposition: one warp per positive + its k negatives (k_score_sampled, oea_transe.cuh), or the octet / duo
+// layouts (8 lanes per row) for the squared-L2 score at pitch <= 128.  The fed scorer (one warp per triple) is
+// oea_triple_score_fed in oea_triple_ext.cu.
 #include <stdlib.h>
 #include "oea_rowmath.cuh"
 #include "oea_rowopt.cuh"
 #include "oea_sampler.cuh"
 #include "oea_duo.cuh"
+#include "oea_transe.cuh"
 #include <cooperative_groups.h>
 
 namespace oea {
-
-// ------------------------------------------------------------------------------------------------
-// Fed path, independent losses (limited / logistic / positive / logsigmoid): one warp per triple.
-// ------------------------------------------------------------------------------------------------
-template <int SCORE, int VEC>
-__global__ void __launch_bounds__(kThreads)
-k_score_fed(TableDev ent, TableDev rel,
-            const int32_t* __restrict__ ph, const int32_t* __restrict__ pr, const int32_t* __restrict__ pt, int n_pos,
-            const int32_t* __restrict__ nh, const int32_t* __restrict__ nr, const int32_t* __restrict__ nt, int n_neg,
-            oea_loss_cfg cfg, double* __restrict__ loss_out) {
-    __shared__ double s_loss[kWarpsPerBlock];
-    const int lane = threadIdx.x & 31;
-    const int warp_global = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
-    const int n_warps = gridDim.x * kWarpsPerBlock;
-    const int total = n_pos + n_neg;
-    float warp_loss = 0.f;
-
-    for (int i = warp_global; i < total; i += n_warps) {
-        const bool is_neg = i >= n_pos;
-        const int j = is_neg ? i - n_pos : i;
-        const int h = is_neg ? __ldg(nh + j) : __ldg(ph + j);
-        const int r = is_neg ? __ldg(nr + j) : __ldg(pr + j);
-        const int t = is_neg ? __ldg(nt + j) : __ldg(pt + j);
-        Row<VEC> xh = load_row<VEC>(ent.w, h, ent.pitch, lane);
-        Row<VEC> xr = load_row<VEC>(rel.w, r, rel.pitch, lane);
-        Row<VEC> xt = load_row<VEC>(ent.w, t, ent.pitch, lane);
-        float ssh = sumsq(xh), ssr = sumsq(xr), sst = sumsq(xt);
-        warp_sum3(ssh, ssr, sst);
-        const float ih = inv_norm(ssh, ent.norm), ir = inv_norm(ssr, rel.norm), it = inv_norm(sst, ent.norm);
-        Row<VEC> u;
-#pragma unroll
-        for (int c = 0; c < VEC; ++c) {
-            xh.v[c] = xh.v[c] * ih; xr.v[c] = xr.v[c] * ir; xt.v[c] = xt.v[c] * it;
-            u.v[c] = xh.v[c] + xr.v[c] - xt.v[c];
-        }
-        const float s = warp_sum(score_partial<SCORE, VEC>(u));
-        float L, g;
-        loss_of(cfg.loss_kind, is_neg, s, cfg, L, g);
-        warp_loss += L;
-        if (g != 0.f) {
-            Row<VEC> du = score_dir<SCORE, VEC>(u);
-#pragma unroll
-            for (int c = 0; c < VEC; ++c) du.v[c] = du.v[c] * g;
-            float dh = dotr(xh, du), dr = dotr(xr, du), dt = dotr(xt, du);
-            warp_sum3(dh, dr, dt);
-            Row<VEC> gh = through_norm(du, xh, dh, ih, ssh, ent.norm);
-            Row<VEC> gr = through_norm(du, xr, dr, ir, ssr, rel.norm);
-            Row<VEC> gt = through_norm(du, xt, dt, it, sst, ent.norm);
-#pragma unroll
-            for (int c = 0; c < VEC; ++c) gt.v[c] = neg(gt.v[c]);
-            red_row<VEC>(ent.g, h, ent.pitch, lane, gh);
-            red_row<VEC>(rel.g, r, rel.pitch, lane, gr);
-            red_row<VEC>(ent.g, t, ent.pitch, lane, gt);
-            if (lane == 0) { ent.touched[h] = 1; rel.touched[r] = 1; ent.touched[t] = 1; }
-        }
-    }
-    LossAcc acc{s_loss};
-    acc.flush(warp_loss, loss_out);
-}
-
-// ------------------------------------------------------------------------------------------------
-// Fed path, margin-based loss Σ relu(m + s⁺_i − s⁻_i) (losses.py:15-27; k = 1): warp per pair.
-// ------------------------------------------------------------------------------------------------
-template <int SCORE, int VEC>
-__global__ void __launch_bounds__(kThreads)
-k_score_margin(TableDev ent, TableDev rel,
-               const int32_t* __restrict__ ph, const int32_t* __restrict__ pr, const int32_t* __restrict__ pt,
-               const int32_t* __restrict__ nh, const int32_t* __restrict__ nr, const int32_t* __restrict__ nt, int n,
-               oea_loss_cfg cfg, double* __restrict__ loss_out) {
-    __shared__ double s_loss[kWarpsPerBlock];
-    const int lane = threadIdx.x & 31;
-    const int warp_global = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
-    const int n_warps = gridDim.x * kWarpsPerBlock;
-    float warp_loss = 0.f;
-
-    for (int i = warp_global; i < n; i += n_warps) {
-        int idx[2][3] = {{__ldg(ph + i), __ldg(pr + i), __ldg(pt + i)}, {__ldg(nh + i), __ldg(nr + i), __ldg(nt + i)}};
-        Row<VEC> xh[2], xr[2], xt[2], u[2];
-        float ih[2], ir[2], it[2], ssh[2], ssr[2], sst[2], s[2];
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-            xh[q] = load_row<VEC>(ent.w, idx[q][0], ent.pitch, lane);
-            xr[q] = load_row<VEC>(rel.w, idx[q][1], rel.pitch, lane);
-            xt[q] = load_row<VEC>(ent.w, idx[q][2], ent.pitch, lane);
-        }
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-            ssh[q] = sumsq(xh[q]); ssr[q] = sumsq(xr[q]); sst[q] = sumsq(xt[q]);
-            warp_sum3(ssh[q], ssr[q], sst[q]);
-            ih[q] = inv_norm(ssh[q], ent.norm); ir[q] = inv_norm(ssr[q], rel.norm); it[q] = inv_norm(sst[q], ent.norm);
-#pragma unroll
-            for (int c = 0; c < VEC; ++c) {
-                xh[q].v[c] = xh[q].v[c] * ih[q]; xr[q].v[c] = xr[q].v[c] * ir[q]; xt[q].v[c] = xt[q].v[c] * it[q];
-                u[q].v[c] = xh[q].v[c] + xr[q].v[c] - xt[q].v[c];
-            }
-            s[q] = score_partial<SCORE, VEC>(u[q]);
-        }
-        warp_sum2(s[0], s[1]);
-        const float v = cfg.margin + s[0] - s[1];
-        warp_loss += fmaxf(v, 0.f);
-        if (v > 0.f) {
-#pragma unroll
-            for (int q = 0; q < 2; ++q) {
-                const float g = q == 0 ? 1.f : -1.f;
-                Row<VEC> du = score_dir<SCORE, VEC>(u[q]);
-#pragma unroll
-                for (int c = 0; c < VEC; ++c) du.v[c] = du.v[c] * g;
-                float dh = dotr(xh[q], du), dr = dotr(xr[q], du), dt = dotr(xt[q], du);
-                warp_sum3(dh, dr, dt);
-                Row<VEC> gh = through_norm(du, xh[q], dh, ih[q], ssh[q], ent.norm);
-                Row<VEC> gr = through_norm(du, xr[q], dr, ir[q], ssr[q], rel.norm);
-                Row<VEC> gt = through_norm(du, xt[q], dt, it[q], sst[q], ent.norm);
-#pragma unroll
-                for (int c = 0; c < VEC; ++c) gt.v[c] = neg(gt.v[c]);
-                red_row<VEC>(ent.g, idx[q][0], ent.pitch, lane, gh);
-                red_row<VEC>(rel.g, idx[q][1], rel.pitch, lane, gr);
-                red_row<VEC>(ent.g, idx[q][2], ent.pitch, lane, gt);
-                if (lane == 0) { ent.touched[idx[q][0]] = 1; rel.touched[idx[q][1]] = 1; ent.touched[idx[q][2]] = 1; }
-            }
-        }
-    }
-    LossAcc acc{s_loss};
-    acc.flush(warp_loss, loss_out);
-}
 
 // ------------------------------------------------------------------------------------------------
 // Fused sampled step: warp per positive; samples its k negatives on device, loads 3 + k rows,
@@ -151,129 +27,12 @@ k_score_margin(TableDev ent, TableDev rel,
 // ------------------------------------------------------------------------------------------------
 template <int SCORE, int VEC>
 __global__ void __launch_bounds__(kThreads)
-k_score_sampled(TableDev ent, TableDev rel, SampledParams P, oea_loss_cfg cfg,
+k_score_sampled(TableDev ent, TableDev rel, const __grid_constant__ SampledParams P, oea_loss_cfg cfg,
                 double* __restrict__ loss_out, int32_t* __restrict__ dbg) {
     __shared__ double s_loss[kWarpsPerBlock];
-    if (P.dev_seed != nullptr) P.seed ^= __ldg(reinterpret_cast<const unsigned long long*>(P.dev_seed));
-    const int lane = threadIdx.x & 31;
-    const int warp_global = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
-    const int n_warps = gridDim.x * kWarpsPerBlock;
-    const int n_pos = P.n_slice[0] + P.n_slice[1];
-    const int k = P.k;
-    float warp_loss = 0.f;
-
-    for (int p = warp_global * P.shard_world + P.shard_rank; p < n_pos; p += n_warps * P.shard_world) {
-        const int q = p < P.n_slice[0] ? 0 : 1;
-        const oea_kg_view& kg = P.kg[q];
-        const int local = q == 0 ? p : p - P.n_slice[0];
-        const uint32_t tri = feistel_perm((uint32_t)(P.start[q] + local), (uint32_t)kg.n_triples,
-                                          P.seed ^ (q ? 0xA5A5A5A5DEADBEEFull : 0x0123456789ABCDEFull));
-        int hrt = 0;
-        if (lane < 3) hrt = __ldg(kg.triples + 3 * (size_t)tri + lane);
-        const int h = __shfl_sync(OEA_FULL, hrt, 0);
-        const int r = __shfl_sync(OEA_FULL, hrt, 1);
-        const int t = __shfl_sync(OEA_FULL, hrt, 2);
-        if (lane < 3) {   // overlap the three shared rows' fetch with the sampling chain
-            const float* rowp = lane == 1 ? rel.w + (size_t)r * rel.pitch : ent.w + (size_t)(lane == 0 ? h : t) * ent.pitch;
-            prefetch_row_l2(rowp, ent.pitch);
-        }
-
-        // ---- negative sampling (batch.py:89-119), lane j < k owns negative j ----
-        int neg_e = 0;
-        bool neg_head = false;
-        warp_sample_negatives(P, P.seed, kg, p, h, r, t, k, lane, ent.w, ent.pitch, neg_e, neg_head);
-        const unsigned head_mask = __ballot_sync(OEA_FULL, neg_head);
-        if (dbg != nullptr) {
-            int32_t* row = dbg + (size_t)p * (2 + k);
-            if (lane == 0) { row[0] = (int32_t)tri + (q ? (1 << 30) : 0); row[1] = (int32_t)head_mask; }
-            if (lane < k) row[2 + lane] = neg_e;
-        }
-
-        // ---- positive triple ----
-        Row<VEC> xh = load_row<VEC>(ent.w, h, ent.pitch, lane);
-        Row<VEC> xr = load_row<VEC>(rel.w, r, rel.pitch, lane);
-        Row<VEC> xt = load_row<VEC>(ent.w, t, ent.pitch, lane);
-        float ssh = sumsq(xh), ssr = sumsq(xr), sst = sumsq(xt);
-        warp_sum3(ssh, ssr, sst);
-        const float ih = inv_norm(ssh, ent.norm), ir = inv_norm(ssr, rel.norm), it = inv_norm(sst, ent.norm);
-        Row<VEC> hr, rt, u, Gh, Gr, Gt;  // hr = ĥ + r̂, rt = r̂ − t̂
-#pragma unroll
-        for (int c = 0; c < VEC; ++c) {
-            xh.v[c] = xh.v[c] * ih; xr.v[c] = xr.v[c] * ir; xt.v[c] = xt.v[c] * it;
-            hr.v[c] = xh.v[c] + xr.v[c];
-            rt.v[c] = xr.v[c] - xt.v[c];
-            u.v[c] = hr.v[c] - xt.v[c];
-        }
-        const float sp = warp_sum(score_partial<SCORE, VEC>(u));
-        const bool margin_mode = cfg.loss_kind == OEA_LOSS_MARGIN;   // Σ relu(m + s⁺ − s⁻), k == 1
-        float L = 0.f, g = 0.f;
-        if (!margin_mode) loss_of(cfg.loss_kind, false, sp, cfg, L, g);
-        warp_loss += L;
-        bool any_grad = g != 0.f;
-        const Row<VEC> dir_pos = score_dir<SCORE, VEC>(u);
-#pragma unroll
-        for (int c = 0; c < VEC; ++c) { Gh.v[c] = dir_pos.v[c] * g; Gr.v[c] = Gh.v[c]; Gt.v[c] = neg(Gh.v[c]); }
-
-        // ---- negatives: only the corrupted row is new ----
-        for (int j = 0; j < k; ++j) {
-            const int e = __shfl_sync(OEA_FULL, neg_e, j);
-            const bool head = (head_mask >> j) & 1u;
-            Row<VEC> xe = load_row<VEC>(ent.w, e, ent.pitch, lane);
-            const float sse = warp_sum(sumsq(xe));
-            const float ie = inv_norm(sse, ent.norm);
-#pragma unroll
-            for (int c = 0; c < VEC; ++c) {
-                xe.v[c] = xe.v[c] * ie;
-                u.v[c] = head ? (xe.v[c] + rt.v[c]) : (hr.v[c] - xe.v[c]);
-            }
-            Row<VEC> dir = score_dir<SCORE, VEC>(u);
-            float sn = score_partial<SCORE, VEC>(u), de = dotr(xe, dir);
-            warp_sum2(sn, de);
-            if (margin_mode) {
-                const float v = cfg.margin + sp - sn;
-                L = fmaxf(v, 0.f);
-                g = v > 0.f ? -1.f : 0.f;
-                if (v > 0.f) {   // the positive's share of the active hinge
-#pragma unroll
-                    for (int c = 0; c < VEC; ++c) { Gh.v[c] = Gh.v[c] + dir_pos.v[c]; Gr.v[c] = Gr.v[c] + dir_pos.v[c]; Gt.v[c] = Gt.v[c] - dir_pos.v[c]; }
-                }
-            } else {
-                loss_of(cfg.loss_kind, true, sn, cfg, L, g);
-            }
-            warp_loss += L;
-            if (g != 0.f) {
-                any_grad = true;
-                const float ge = head ? g : -g;  // d/dê = ±g·dir
-                Row<VEC> Ge;
-#pragma unroll
-                for (int c = 0; c < VEC; ++c) {
-                    const float4 du = dir.v[c] * g;
-                    Gr.v[c] = Gr.v[c] + du;
-                    if (head) Gt.v[c] = Gt.v[c] - du; else Gh.v[c] = Gh.v[c] + du;
-                    Ge.v[c] = dir.v[c] * ge;
-                }
-                Row<VEC> out = through_norm(Ge, xe, ge * de, ie, sse, ent.norm);
-                red_row<VEC>(ent.g, e, ent.pitch, lane, out);
-                if (lane == 0) ent.touched[e] = 1;
-            }
-        }
-
-        if (any_grad) {
-            float dh = dotr(xh, Gh), dr = dotr(xr, Gr), dt = dotr(xt, Gt);
-            warp_sum3(dh, dr, dt);
-            Row<VEC> oh = through_norm(Gh, xh, dh, ih, ssh, ent.norm);
-            Row<VEC> orr = through_norm(Gr, xr, dr, ir, ssr, rel.norm);
-            Row<VEC> ot = through_norm(Gt, xt, dt, it, sst, ent.norm);
-            red_row<VEC>(ent.g, h, ent.pitch, lane, oh);
-            red_row<VEC>(rel.g, r, rel.pitch, lane, orr);
-            red_row<VEC>(ent.g, t, ent.pitch, lane, ot);
-            if (lane == 0) { ent.touched[h] = 1; rel.touched[r] = 1; ent.touched[t] = 1; }
-        }
-    }
-    LossAcc acc{s_loss};
-    acc.flush(warp_loss, loss_out);
+    const FedBatch none{};
+    positive_score_body<SCORE, VEC, false>(ent, rel, P, none, cfg, loss_out, dbg, s_loss);
 }
-
 
 // ------------------------------------------------------------------------------------------------
 // Fused sampled step, v2 ("octet" layout) for the squared-L2 score and pitch <= 128 floats:
@@ -555,54 +314,48 @@ k_step_sampled_duo(TableDev ent, TableDev rel, const __grid_constant__ SampledPa
 }
 
 // ------------------------------------------------------------------------------------------------
-// Row optimiser: one warp per row, flagged rows only (Adagrad / SGD) or all rows (Adam).
-// TF1 semantics (optimizers.py:10-20): Adagrad acc += g², x −= lr·g/√acc (no ε, acc0 = 0.1 set by
-// the caller); Adam lr_t = lr·√(1−β2^t)/(1−β1^t), x −= lr_t·m/(√v + ε).
+// Adam (optimizers.py:10-20), the one dense rule: one warp per row, every row.  TF1 semantics:
+// lr_t = lr·√(1−β2^t)/(1−β1^t), x −= lr_t·m/(√v + ε).  Adagrad / SGD update the flagged rows only
+// (k_rowopt_pair below).
 // ------------------------------------------------------------------------------------------------
-template <int KIND>
 __global__ void __launch_bounds__(kThreads)
-k_rowopt(float* __restrict__ w, float* __restrict__ grad, float* __restrict__ s1, float* __restrict__ s2,
-         int32_t* __restrict__ touched, int rows, int pitch, float lr, float beta1, float beta2, float eps,
-         float lr_t) {
+k_rowopt_adam(float* __restrict__ w, float* __restrict__ grad, float* __restrict__ s1, float* __restrict__ s2,
+              int32_t* __restrict__ touched, int rows, int pitch, float beta1, float beta2, float eps, float lr_t) {
     const int lane = threadIdx.x & 31;
     const int warp_global = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
     const int n_warps = gridDim.x * kWarpsPerBlock;
     const int p4 = pitch >> 2;
     for (int row = warp_global; row < rows; row += n_warps) {
-        if (KIND != OEA_OPT_ADAM) {
-            if (touched[row] == 0) continue;
-        }
         const size_t base = (size_t)row * pitch;
         for (int c = lane; c < p4; c += OEA_WARP) {
             const size_t o = base + 4 * (size_t)c;
             float4 g = *reinterpret_cast<float4*>(grad + o);
             float4 x = *reinterpret_cast<float4*>(w + o);
-            if (KIND == OEA_OPT_ADAGRAD) {
-                float4 a = *reinterpret_cast<float4*>(s1 + o);
-                a.x = fmaf(g.x, g.x, a.x); a.y = fmaf(g.y, g.y, a.y); a.z = fmaf(g.z, g.z, a.z); a.w = fmaf(g.w, g.w, a.w);
-                x.x -= lr * g.x * rsqrtf(a.x); x.y -= lr * g.y * rsqrtf(a.y);
-                x.z -= lr * g.z * rsqrtf(a.z); x.w -= lr * g.w * rsqrtf(a.w);
-                *reinterpret_cast<float4*>(s1 + o) = a;
-            } else if (KIND == OEA_OPT_SGD) {
-                x.x -= lr * g.x; x.y -= lr * g.y; x.z -= lr * g.z; x.w -= lr * g.w;
-            } else {
-                float4 m = *reinterpret_cast<float4*>(s1 + o);
-                float4 v = *reinterpret_cast<float4*>(s2 + o);
-                m.x = beta1 * m.x + (1.f - beta1) * g.x; m.y = beta1 * m.y + (1.f - beta1) * g.y;
-                m.z = beta1 * m.z + (1.f - beta1) * g.z; m.w = beta1 * m.w + (1.f - beta1) * g.w;
-                v.x = beta2 * v.x + (1.f - beta2) * g.x * g.x; v.y = beta2 * v.y + (1.f - beta2) * g.y * g.y;
-                v.z = beta2 * v.z + (1.f - beta2) * g.z * g.z; v.w = beta2 * v.w + (1.f - beta2) * g.w * g.w;
-                x.x -= lr_t * m.x / (sqrtf(v.x) + eps); x.y -= lr_t * m.y / (sqrtf(v.y) + eps);
-                x.z -= lr_t * m.z / (sqrtf(v.z) + eps); x.w -= lr_t * m.w / (sqrtf(v.w) + eps);
-                *reinterpret_cast<float4*>(s1 + o) = m;
-                *reinterpret_cast<float4*>(s2 + o) = v;
-            }
+            float4 m = *reinterpret_cast<float4*>(s1 + o);
+            float4 v = *reinterpret_cast<float4*>(s2 + o);
+            m.x = beta1 * m.x + (1.f - beta1) * g.x; m.y = beta1 * m.y + (1.f - beta1) * g.y;
+            m.z = beta1 * m.z + (1.f - beta1) * g.z; m.w = beta1 * m.w + (1.f - beta1) * g.w;
+            v.x = beta2 * v.x + (1.f - beta2) * g.x * g.x; v.y = beta2 * v.y + (1.f - beta2) * g.y * g.y;
+            v.z = beta2 * v.z + (1.f - beta2) * g.z * g.z; v.w = beta2 * v.w + (1.f - beta2) * g.w * g.w;
+            x.x -= lr_t * m.x / (sqrtf(v.x) + eps); x.y -= lr_t * m.y / (sqrtf(v.y) + eps);
+            x.z -= lr_t * m.z / (sqrtf(v.z) + eps); x.w -= lr_t * m.w / (sqrtf(v.w) + eps);
+            *reinterpret_cast<float4*>(s1 + o) = m;
+            *reinterpret_cast<float4*>(s2 + o) = v;
             *reinterpret_cast<float4*>(w + o) = x;
             *reinterpret_cast<float4*>(grad + o) = f4(0.f);
         }
-        __syncwarp();      // every lane has read the flag (above) before lane 0 clears it: no reliance on convergence
+        __syncwarp();
         if (lane == 0) touched[row] = 0;
     }
+}
+
+// Adagrad / SGD over the concatenated row space [A rows | B rows] (same pitch), flagged rows only
+// (rowopt_flagged_body, the optimiser phase of the one-launch steps, on a grid of its own).  One table is (t, a table
+// of no rows).
+template <int KIND>
+__global__ void __launch_bounds__(kThreads)
+k_rowopt_pair(OptTab A, OptTab B, int pitch, float lr) {
+    rowopt_flagged_body<KIND>(A, B, pitch, lr, blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5), gridDim.x * kWarpsPerBlock);
 }
 
 // Normalised lookup: out[i] = normalise(weight[ids[i]]) (basic_model.py:106-121 `.eval()` reads).
@@ -647,58 +400,20 @@ extern "C" const char* oea_error_string(int code) {
     }
 }
 
-extern "C" int oea_triple_score_fed(const oea_table* ent, const oea_table* rel,
-                                    const int32_t* pos_h, const int32_t* pos_r, const int32_t* pos_t, int32_t n_pos,
-                                    const int32_t* neg_h, const int32_t* neg_r, const int32_t* neg_t, int32_t n_neg,
-                                    const oea_loss_cfg* loss, double* loss_out, void* stream) {
-    int rc = check_table(ent, true); if (rc) return rc;
-    rc = check_table(rel, true); if (rc) return rc;
-    if (loss == nullptr || loss_out == nullptr) return OEA_ERR_NULL;
-    if (n_pos < 0 || n_neg < 0) return OEA_ERR_SHAPE;
-    if (n_pos > 0 && (!pos_h || !pos_r || !pos_t)) return OEA_ERR_NULL;
-    if (n_neg > 0 && (!neg_h || !neg_r || !neg_t)) return OEA_ERR_NULL;
-    if (ent->pitch != rel->pitch || ent->dim != rel->dim) return OEA_ERR_DIM;
-    if (loss->score_kind != OEA_SCORE_L1 && loss->score_kind != OEA_SCORE_L2SQ) return OEA_ERR_KIND;
-    if (loss->loss_kind < OEA_LOSS_MARGIN || loss->loss_kind > OEA_LOSS_LOGSIGMOID) return OEA_ERR_KIND;
-    if (loss->loss_kind == OEA_LOSS_MARGIN && n_neg != n_pos) return OEA_ERR_SHAPE;  // args_hander.py:19-21
-    if ((loss->loss_kind == OEA_LOSS_POSITIVE || loss->loss_kind == OEA_LOSS_LOGSIGMOID) && n_neg != 0) return OEA_ERR_SHAPE;
-    if (n_pos + n_neg == 0) return OEA_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    TableDev e = table_dev(ent), r = table_dev(rel);
-    const bool l1 = loss->score_kind == OEA_SCORE_L1;
-    if (loss->loss_kind == OEA_LOSS_MARGIN) {
-        const int grid = grid_for(n_pos);
-#define CALL(V)                                                                                                         \
-        if (l1) OEA_LAUNCH((k_score_margin<OEA_SCORE_L1, V>), grid, kThreads, 0, st, e, r, pos_h, pos_r, pos_t, neg_h, neg_r, neg_t, n_pos, *loss, loss_out); \
-        else OEA_LAUNCH((k_score_margin<OEA_SCORE_L2SQ, V>), grid, kThreads, 0, st, e, r, pos_h, pos_r, pos_t, neg_h, neg_r, neg_t, n_pos, *loss, loss_out)
-        OEA_DISPATCH_VEC(ent->pitch, CALL);
-#undef CALL
-    } else {
-#define CALL(V)                                                                                                         \
-        if (l1) { const int grid = grid_one_wave<k_score_fed<OEA_SCORE_L1, V>>(n_pos + n_neg);                              \
-                  OEA_LAUNCH((k_score_fed<OEA_SCORE_L1, V>), grid, kThreads, 0, st, e, r, pos_h, pos_r, pos_t, n_pos, neg_h, neg_r, neg_t, n_neg, *loss, loss_out); } \
-        else { const int grid = grid_one_wave<k_score_fed<OEA_SCORE_L2SQ, V>>(n_pos + n_neg);                               \
-               OEA_LAUNCH((k_score_fed<OEA_SCORE_L2SQ, V>), grid, kThreads, 0, st, e, r, pos_h, pos_r, pos_t, n_pos, neg_h, neg_r, neg_t, n_neg, *loss, loss_out); }
-        OEA_DISPATCH_VEC(ent->pitch, CALL);
-#undef CALL
-    }
-    OEA_LAUNCH_CHECK();
-    return OEA_OK;
-}
-
 extern "C" int oea_rowopt_apply(const oea_table* t, const oea_opt_cfg* opt, void* stream) {
     int rc = check_table(t, true); if (rc) return rc;
     if (opt == nullptr) return OEA_ERR_NULL;
     cudaStream_t st = (cudaStream_t)stream;
-    const int grid = grid_for(t->rows);
     switch (opt->kind) {
         case OEA_OPT_ADAGRAD:
-            if (!t->state1) return OEA_ERR_NULL;
-            OEA_LAUNCH(k_rowopt<OEA_OPT_ADAGRAD>, grid, kThreads, 0, st, t->weight, t->grad, t->state1, nullptr, t->touched, t->rows, t->pitch, opt->lr, 0.f, 0.f, 0.f, 0.f);
+        case OEA_OPT_SGD: {   // the flagged-row body over (t, an empty second table)
+            if (opt->kind == OEA_OPT_ADAGRAD && !t->state1) return OEA_ERR_NULL;
+            const OptTab A{t->weight, t->grad, t->state1, t->touched, t->rows}, none{nullptr, nullptr, nullptr, nullptr, 0};
+            const int grid = grid_for((t->rows + 3) / 4);
+            if (opt->kind == OEA_OPT_ADAGRAD) OEA_LAUNCH(k_rowopt_pair<OEA_OPT_ADAGRAD>, grid, kThreads, 0, st, A, none, t->pitch, opt->lr);
+            else OEA_LAUNCH(k_rowopt_pair<OEA_OPT_SGD>, grid, kThreads, 0, st, A, none, t->pitch, opt->lr);
             break;
-        case OEA_OPT_SGD:
-            OEA_LAUNCH(k_rowopt<OEA_OPT_SGD>, grid, kThreads, 0, st, t->weight, t->grad, nullptr, nullptr, t->touched, t->rows, t->pitch, opt->lr, 0.f, 0.f, 0.f, 0.f);
-            break;
+        }
         case OEA_OPT_ADADELTA:
             return oea_rowopt_adadelta(t, opt, stream);   // oea_optim_ext.cu
         case OEA_OPT_ADAM: {
@@ -707,7 +422,7 @@ extern "C" int oea_rowopt_apply(const oea_table* t, const oea_opt_cfg* opt, void
             const double b1t = 1.0 - pow((double)opt->beta1, (double)opt->t);
             const double b2t = 1.0 - pow((double)opt->beta2, (double)opt->t);
             const float lr_t = (float)((double)opt->lr * sqrt(b2t) / b1t);
-            OEA_LAUNCH(k_rowopt<OEA_OPT_ADAM>, grid, kThreads, 0, st, t->weight, t->grad, t->state1, t->state2, t->touched, t->rows, t->pitch, opt->lr, opt->beta1, opt->beta2, opt->eps, lr_t);
+            OEA_LAUNCH(k_rowopt_adam, grid_for(t->rows), kThreads, 0, st, t->weight, t->grad, t->state1, t->state2, t->touched, t->rows, t->pitch, opt->beta1, opt->beta2, opt->eps, lr_t);
             break;
         }
         default:
@@ -776,49 +491,6 @@ extern "C" int oea_triple_score_sampled(const oea_table* ent, const oea_table* r
 #undef CALL
     }
     OEA_LAUNCH_CHECK();
-    return OEA_OK;
-}
-
-extern "C" int oea_rowopt_apply_pair(const oea_table* a, const oea_table* b, const oea_opt_cfg* opt, void* stream);
-
-extern "C" int oea_triple_step_fed_host(const oea_table* ent, const oea_table* rel,
-                                        const int32_t* pos_hrt_host, int32_t n_pos,
-                                        const int32_t* neg_hrt_host, int32_t n_neg,
-                                        const oea_loss_cfg* loss, const oea_opt_cfg* opt,
-                                        int32_t* dev_idx_ws, double* dev_loss_ws, double* loss_pinned_host,
-                                        float* loss_host, void* stream) {
-    if (!dev_idx_ws || !dev_loss_ws || !loss_pinned_host || !loss_host || !opt) return OEA_ERR_NULL;
-    if (n_pos < 0 || n_neg < 0) return OEA_ERR_SHAPE;
-    if ((n_pos > 0 && !pos_hrt_host) || (n_neg > 0 && !neg_hrt_host)) return OEA_ERR_NULL;
-    cudaStream_t st = (cudaStream_t)stream;
-    int32_t* dpos = dev_idx_ws;
-    int32_t* dneg = dev_idx_ws + 3 * (size_t)n_pos;
-    if (n_pos) OEA_CUDA_TRY(cudaMemcpyAsync(dpos, pos_hrt_host, 3 * (size_t)n_pos * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    if (n_neg) OEA_CUDA_TRY(cudaMemcpyAsync(dneg, neg_hrt_host, 3 * (size_t)n_neg * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    OEA_CUDA_TRY(cudaMemsetAsync(dev_loss_ws, 0, sizeof(double), st));
-    // OEA_FED_GROUPED=1: score a positive together with its negatives when the batch has the reference's layout
-    // (oea_triple_grouped.cu; opt-in until it has been timed on hardware)
-    const char* grouped_env = getenv("OEA_FED_GROUPED");
-    const bool grouped = grouped_env && grouped_env[0] == '1' && n_pos > 0 && n_neg % n_pos == 0;
-    // OEA_FED_FUSED=1: grouped scoring and the row optimiser as one cooperative launch where that kernel applies
-    const char* fused_env = getenv("OEA_FED_FUSED");
-    int rc = OEA_ERR_KIND;
-    if (fused_env && fused_env[0] == '1' && n_pos > 0 && n_neg % n_pos == 0)
-        rc = oea_triple_step_fed_grouped(ent, rel, dpos, dpos + n_pos, dpos + 2 * (size_t)n_pos, n_pos,
-                                         dneg, dneg + n_neg, dneg + 2 * (size_t)n_neg, n_neg, loss, opt, dev_loss_ws, stream);
-    if (rc == OEA_ERR_KIND) {
-        rc = grouped
-            ? oea_triple_score_fed_grouped(ent, rel, dpos, dpos + n_pos, dpos + 2 * (size_t)n_pos, n_pos,
-                                           dneg, dneg + n_neg, dneg + 2 * (size_t)n_neg, n_neg, loss, dev_loss_ws, stream)
-            : oea_triple_score_fed(ent, rel, dpos, dpos + n_pos, dpos + 2 * (size_t)n_pos, n_pos,
-                                   dneg, dneg + n_neg, dneg + 2 * (size_t)n_neg, n_neg, loss, dev_loss_ws, stream);
-        if (rc) return rc;
-        rc = oea_rowopt_apply_pair(ent, rel, opt, stream);
-    }
-    if (rc) return rc;
-    OEA_CUDA_TRY(cudaMemcpyAsync(loss_pinned_host, dev_loss_ws, sizeof(double), cudaMemcpyDeviceToHost, st));
-    OEA_CUDA_TRY(cudaStreamSynchronize(st));
-    *loss_host = (float)(*loss_pinned_host);
     return OEA_OK;
 }
 
@@ -1080,19 +752,6 @@ extern "C" int oea_mapping_fwd_bwd(const float* e1, const float* e2, int32_t n, 
 // ================================================================================================
 // One call per training step: fused sampler+scorer, then ONE row-optimiser launch over both tables.
 // ================================================================================================
-namespace oea {
-
-
-// Adagrad / SGD over the concatenated row space [ent rows | rel rows] (same pitch), flagged rows only
-// (rowopt_flagged_body, the optimiser phase of the one-launch steps, on a grid of its own).
-template <int KIND>
-__global__ void __launch_bounds__(kThreads)
-k_rowopt_pair(OptTab A, OptTab B, int pitch, float lr) {
-    rowopt_flagged_body<KIND>(A, B, pitch, lr, blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5), gridDim.x * kWarpsPerBlock);
-}
-
-}  // namespace oea
-
 extern "C" int oea_rowopt_apply_pair(const oea_table* a, const oea_table* b, const oea_opt_cfg* opt, void* stream) {
     int rc = check_table(a, true); if (rc) return rc;
     rc = check_table(b, true); if (rc) return rc;

@@ -1,8 +1,9 @@
-// oea_triple_ext.cu — path (i), SURVEY §8f-2: the other score functions of the reference's models/ on the
-// fed boundary (index vectors in, gradients scattered into the tables), one warp per triple.  sm_90a.
+// oea_triple_ext.cu — path (i), SURVEY §8f-2: the score functions of the reference's models/ on the fed boundary
+// (index vectors in, gradients scattered into the tables), one warp per triple.  sm_90a.
 //
 // Maths restated from the reference (no code shared):
-//   models/trans/transh.py:25-51        TransH   e⊥ = e − <e, n̂> n̂,  n̂ = l2_normalize(normal_vector[r])
+//   models/trans/transe.py:33-45       TransE   ĥ + r̂ − t̂ (oea_transe.cuh; also oea_triple_score_fed, pitch <= 512)
+//   models/trans/transh.py:25-51       TransH   e⊥ = e − <e, n̂> n̂,  n̂ = l2_normalize(normal_vector[r])
 //   approaches/bootea_transh.py:57-95   the same projection under the limited loss
 //   models/trans/transd.py:26-65        TransD   e⊥ = l2_normalize(e + <e, e_p> r_p)
 //   models/semantic/distmult.py:43-59   DistMult score Σ h∘r∘t, softplus(−label·score), reduce_mean
@@ -32,42 +33,11 @@
 //     0 … 2d−1, so that i + k never needs a modulo) in this warp's shared memory, and lane l owns the output
 //     coordinates k = l, l + 32, …  The index wraps modulo dim, never pitch.  HolE trains with the margin loss over the
 //     reference batch layout (negatives of positive p at p·k … p·k+k−1, their energies averaged): k_hole_margin.
-#include "oea_rowmath.cuh"
+#include "oea_transe.cuh"
 
 namespace oea {
 
-struct ModelDev {
-    TableDev ent, rel, ent_aux, rel_aux;
-    int dim;                 // columns that carry data (HolE's correlation wraps modulo dim)
-    float gamma, phase;      // RotatE: γ and the phase scale π/ρ (oea_model.gamma / .phase); unused by the other kinds
-};
-
-// ---- one triple of each model ------------------------------------------------------------------------------------
-template <int MODEL, int SCORE, int VEC>
-struct Triple;
-
-// TransE (models/trans/transe.py:33-45): the family's base case; also cross-checks this file against oea_triple.cu
-template <int SCORE, int VEC>
-struct Triple<OEA_MODEL_TRANSE, SCORE, VEC> {
-    int h, r, t;
-    NRow<VEC> xh, xr, xt;
-    Row<VEC> u;
-    __device__ __forceinline__ float forward(const ModelDev& M, int h_, int r_, int t_, int lane) {
-        h = h_; r = r_; t = t_;
-        xh = lookup<VEC>(M.ent, h, lane);
-        xr = lookup<VEC>(M.rel, r, lane);
-        xt = lookup<VEC>(M.ent, t, lane);
-        u = r_sub(r_add(xh.x, xr.x), xt.x);
-        return warp_sum(score_partial<SCORE, VEC>(u));
-    }
-    __device__ __forceinline__ void backward(const ModelDev& M, float g, int lane) {
-        const Row<VEC> du = r_scale(score_dir<SCORE, VEC>(u), g);
-        push<VEC>(M.ent, h, lane, du, xh);
-        push<VEC>(M.rel, r, lane, du, xr);
-        push<VEC>(M.ent, t, lane, r_neg(du), xt);
-    }
-};
-
+// ---- one triple of each model (TransE, the base case, is in oea_transe.cuh) ----------------------------------------
 // TransH: u = ĥ + r̂ − t̂ − (a − b)·n̂ with a = <ĥ, n̂>, b = <t̂, n̂>; rel_aux = normal_vector
 template <int SCORE, int VEC>
 struct Triple<OEA_MODEL_TRANSH, SCORE, VEC> {
@@ -410,8 +380,17 @@ k_model_margin(ModelDev M,
     float warp_loss = 0.f;
     for (int i = warp_global; i < n; i += n_warps) {
         Triple<MODEL, SCORE, VEC> P, N;
-        const float ep = P.forward(M, __ldg(ph + i), __ldg(pr + i), __ldg(pt + i), lane);
-        const float en = N.forward(M, __ldg(nh + i), __ldg(nr + i), __ldg(nt + i), lane);
+        float ep, en;
+        if constexpr (MODEL == OEA_MODEL_TRANSE) {      // six row loads in flight before the first reduction
+            P.gather(M, __ldg(ph + i), __ldg(pr + i), __ldg(pt + i), lane);
+            N.gather(M, __ldg(nh + i), __ldg(nr + i), __ldg(nt + i), lane);
+            ep = P.score(M);
+            en = N.score(M);
+            warp_sum2(ep, en);
+        } else {
+            ep = P.forward(M, __ldg(ph + i), __ldg(pr + i), __ldg(pt + i), lane);
+            en = N.forward(M, __ldg(nh + i), __ldg(nr + i), __ldg(nt + i), lane);
+        }
         const float v = cfg.margin + ep - en;
         warp_loss += fmaxf(v, 0.f) * scale;
         if (v > 0.f) {
@@ -586,6 +565,47 @@ extern "C" int oea_model_score_fed(const oea_model* model,
 #undef OEA_LAUNCH_VEC
 #undef OEA_LAUNCH_MODEL
 #undef OEA_RUN
+    OEA_LAUNCH_CHECK();
+    return OEA_OK;
+}
+
+// TransE with the tables of the call (path (i)'s fed scorer): the kernels above at every pitch up to 512.
+extern "C" int oea_triple_score_fed(const oea_table* ent, const oea_table* rel,
+                                    const int32_t* pos_h, const int32_t* pos_r, const int32_t* pos_t, int32_t n_pos,
+                                    const int32_t* neg_h, const int32_t* neg_r, const int32_t* neg_t, int32_t n_neg,
+                                    const oea_loss_cfg* loss, double* loss_out, void* stream) {
+    int rc = check_table(ent, true); if (rc) return rc;
+    rc = check_table(rel, true); if (rc) return rc;
+    if (loss == nullptr || loss_out == nullptr) return OEA_ERR_NULL;
+    if (n_pos < 0 || n_neg < 0) return OEA_ERR_SHAPE;
+    if (n_pos > 0 && (!pos_h || !pos_r || !pos_t)) return OEA_ERR_NULL;
+    if (n_neg > 0 && (!neg_h || !neg_r || !neg_t)) return OEA_ERR_NULL;
+    if (ent->pitch != rel->pitch || ent->dim != rel->dim) return OEA_ERR_DIM;
+    if (loss->score_kind != OEA_SCORE_L1 && loss->score_kind != OEA_SCORE_L2SQ) return OEA_ERR_KIND;
+    if (loss->loss_kind < OEA_LOSS_MARGIN || loss->loss_kind > OEA_LOSS_LOGSIGMOID) return OEA_ERR_KIND;
+    if (loss->loss_kind == OEA_LOSS_MARGIN && n_neg != n_pos) return OEA_ERR_SHAPE;  // args_hander.py:19-21
+    if ((loss->loss_kind == OEA_LOSS_POSITIVE || loss->loss_kind == OEA_LOSS_LOGSIGMOID) && n_neg != 0) return OEA_ERR_SHAPE;
+    if (n_pos + n_neg == 0) return OEA_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    const TableDev e = table_dev(ent), r = table_dev(rel);
+    const ModelDev M{e, r, e, r, ent->dim, 0.f, 0.f};
+    const bool l1 = loss->score_kind == OEA_SCORE_L1;
+    if (loss->loss_kind == OEA_LOSS_MARGIN) {
+        const int grid = grid_for(n_pos);
+#define CALL(V)                                                                                                         \
+        if (l1) OEA_LAUNCH((k_model_margin<OEA_MODEL_TRANSE, OEA_SCORE_L1, V>), grid, kThreads, 0, st, M, pos_h, pos_r, pos_t, neg_h, neg_r, neg_t, n_pos, *loss, 1.f, loss_out); \
+        else OEA_LAUNCH((k_model_margin<OEA_MODEL_TRANSE, OEA_SCORE_L2SQ, V>), grid, kThreads, 0, st, M, pos_h, pos_r, pos_t, neg_h, neg_r, neg_t, n_pos, *loss, 1.f, loss_out)
+        OEA_DISPATCH_VEC(ent->pitch, CALL);
+#undef CALL
+    } else {
+#define CALL(V)                                                                                                         \
+        if (l1) { const int grid = grid_one_wave<k_model_fed<OEA_MODEL_TRANSE, OEA_SCORE_L1, V>>(n_pos + n_neg);        \
+                  OEA_LAUNCH((k_model_fed<OEA_MODEL_TRANSE, OEA_SCORE_L1, V>), grid, kThreads, 0, st, M, pos_h, pos_r, pos_t, n_pos, neg_h, neg_r, neg_t, n_neg, *loss, 1.f, loss_out); } \
+        else { const int grid = grid_one_wave<k_model_fed<OEA_MODEL_TRANSE, OEA_SCORE_L2SQ, V>>(n_pos + n_neg);         \
+               OEA_LAUNCH((k_model_fed<OEA_MODEL_TRANSE, OEA_SCORE_L2SQ, V>), grid, kThreads, 0, st, M, pos_h, pos_r, pos_t, n_pos, neg_h, neg_r, neg_t, n_neg, *loss, 1.f, loss_out); }
+        OEA_DISPATCH_VEC(ent->pitch, CALL);
+#undef CALL
+    }
     OEA_LAUNCH_CHECK();
     return OEA_OK;
 }

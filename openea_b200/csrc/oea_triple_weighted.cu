@@ -10,61 +10,18 @@
 //   k_pair_distance           scale · Σ_i w_i · ‖ê_a(i) − ê_b(i)‖²
 //       IMUSE's align loss over the entity pairs its string matcher found (approaches/imuse.py:303-306).
 //
-// Same row arithmetic, normalisation Jacobian and loss accumulation as oea_triple.cu (oea_rowmath.cuh); one warp per
-// pair, the six (two) rows of a pair in registers.  HBM / L2 bound: 6·4·d B gathered per pair, up to as much reduced.
-// sm_90a.
-#include "oea_rowmath.cuh"
+// k_score_margin_weighted scores a pair with the TransE triple of oea_transe.cuh; k_pair_distance uses the same row
+// arithmetic and normalisation Jacobian (oea_rowmath.cuh).  One warp per pair, the six (two) rows of a pair in
+// registers.  HBM / L2 bound: 6·4·d B gathered per pair, up to as much reduced.  sm_90a.
+#include "oea_transe.cuh"
 
 using namespace oea;
 
 namespace {
 
-template <int VEC>
-struct Triple3 {
-    Row<VEC> xh, xr, xt, u;     // normalised rows and ĥ + r̂ − t̂
-    float ih, ir, it, ssh, ssr, sst;
-};
-
-template <int SCORE, int VEC>
-__device__ __forceinline__ float load_and_score(const TableDev& ent, const TableDev& rel, int h, int r, int t, int lane,
-                                                Triple3<VEC>& T) {
-    T.xh = load_row<VEC>(ent.w, h, ent.pitch, lane);
-    T.xr = load_row<VEC>(rel.w, r, rel.pitch, lane);
-    T.xt = load_row<VEC>(ent.w, t, ent.pitch, lane);
-    T.ssh = sumsq(T.xh); T.ssr = sumsq(T.xr); T.sst = sumsq(T.xt);
-    warp_sum3(T.ssh, T.ssr, T.sst);
-    T.ih = inv_norm(T.ssh, ent.norm); T.ir = inv_norm(T.ssr, rel.norm); T.it = inv_norm(T.sst, ent.norm);
-#pragma unroll
-    for (int c = 0; c < VEC; ++c) {
-        T.xh.v[c] = T.xh.v[c] * T.ih; T.xr.v[c] = T.xr.v[c] * T.ir; T.xt.v[c] = T.xt.v[c] * T.it;
-        T.u.v[c] = T.xh.v[c] + T.xr.v[c] - T.xt.v[c];
-    }
-    return score_partial<SCORE, VEC>(T.u);      // lane partial: the caller reduces
-}
-
-// d(g · s)/d(raw rows) of one triple into the gradient tables
-template <int SCORE, int VEC>
-__device__ __forceinline__ void push_grad(const TableDev& ent, const TableDev& rel, int h, int r, int t, int lane,
-                                          const Triple3<VEC>& T, float g) {
-    Row<VEC> du = score_dir<SCORE, VEC>(T.u);
-#pragma unroll
-    for (int c = 0; c < VEC; ++c) du.v[c] = du.v[c] * g;
-    float dh = dotr(T.xh, du), dr = dotr(T.xr, du), dt = dotr(T.xt, du);
-    warp_sum3(dh, dr, dt);
-    Row<VEC> gh = through_norm(du, T.xh, dh, T.ih, T.ssh, ent.norm);
-    Row<VEC> gr = through_norm(du, T.xr, dr, T.ir, T.ssr, rel.norm);
-    Row<VEC> gt = through_norm(du, T.xt, dt, T.it, T.sst, ent.norm);
-#pragma unroll
-    for (int c = 0; c < VEC; ++c) gt.v[c] = neg(gt.v[c]);
-    red_row<VEC>(ent.g, h, ent.pitch, lane, gh);
-    red_row<VEC>(rel.g, r, rel.pitch, lane, gr);
-    red_row<VEC>(ent.g, t, ent.pitch, lane, gt);
-    if (lane == 0) { ent.touched[h] = 1; rel.touched[r] = 1; ent.touched[t] = 1; }
-}
-
 template <int SCORE, int VEC>
 __global__ void __launch_bounds__(kThreads)
-k_score_margin_weighted(TableDev ent, TableDev rel,
+k_score_margin_weighted(ModelDev M,
                         const int32_t* __restrict__ ph, const int32_t* __restrict__ pr, const int32_t* __restrict__ pt,
                         const int32_t* __restrict__ nh, const int32_t* __restrict__ nr, const int32_t* __restrict__ nt,
                         int n, const float* __restrict__ weights, int reciprocal, float scale, float margin,
@@ -76,20 +33,19 @@ k_score_margin_weighted(TableDev ent, TableDev rel,
     float warp_loss = 0.f;
 
     for (int i = warp_global; i < n; i += n_warps) {
-        const int h0 = __ldg(ph + i), r0 = __ldg(pr + i), t0 = __ldg(pt + i);
-        const int h1 = __ldg(nh + i), r1 = __ldg(nr + i), t1 = __ldg(nt + i);
         float w = weights != nullptr ? __ldg(weights + i) : 1.f;
         if (reciprocal) w = 1.f / w;                       // tf.cast(1 / weight, tf.float32), iptranse.py:179
         w *= scale;
-        Triple3<VEC> P, N;
-        float sp = load_and_score<SCORE, VEC>(ent, rel, h0, r0, t0, lane, P);
-        float sn = load_and_score<SCORE, VEC>(ent, rel, h1, r1, t1, lane, N);
+        Triple<OEA_MODEL_TRANSE, SCORE, VEC> P, N;
+        P.gather(M, __ldg(ph + i), __ldg(pr + i), __ldg(pt + i), lane);
+        N.gather(M, __ldg(nh + i), __ldg(nr + i), __ldg(nt + i), lane);
+        float sp = P.score(M), sn = N.score(M);
         warp_sum2(sp, sn);
         const float v = margin + sp - sn;
         warp_loss += w * fmaxf(v, 0.f);
-        if (v > 0.f && w != 0.f) {                         // relu'(0) = 0 as TF
-            push_grad<SCORE, VEC>(ent, rel, h0, r0, t0, lane, P, w);
-            push_grad<SCORE, VEC>(ent, rel, h1, r1, t1, lane, N, -w);
+        if (v > 0.f && w != 0.f) {                         // relu'(0) = 0 as TF; a zero-weight pair flags no row
+            P.backward(M, w, lane);
+            N.backward(M, -w, lane);
         }
     }
     LossAcc acc{s_loss};
@@ -157,14 +113,15 @@ extern "C" int oea_triple_score_margin_weighted(const oea_table* ent, const oea_
     if (weight_mode != OEA_WEIGHT_DIRECT && weight_mode != OEA_WEIGHT_RECIPROCAL) return OEA_ERR_KIND;
     if (n == 0) return OEA_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    TableDev e = table_dev(ent), r = table_dev(rel);
+    const TableDev e = table_dev(ent), r = table_dev(rel);
+    const ModelDev M{e, r, e, r, ent->dim, 0.f, 0.f};
     const bool l1 = loss->score_kind == OEA_SCORE_L1;
     const int grid = grid_for(n);
     const int recip = weight_mode == OEA_WEIGHT_RECIPROCAL && weights != nullptr;
 #define CALL(V)                                                                                                           \
-    if (l1) OEA_LAUNCH((k_score_margin_weighted<OEA_SCORE_L1, V>), grid, kThreads, 0, st, e, r, pos_h, pos_r, pos_t, neg_h,    \
+    if (l1) OEA_LAUNCH((k_score_margin_weighted<OEA_SCORE_L1, V>), grid, kThreads, 0, st, M, pos_h, pos_r, pos_t, neg_h,    \
                        neg_r, neg_t, n, weights, recip, scale, loss->margin, loss_out);                                       \
-    else OEA_LAUNCH((k_score_margin_weighted<OEA_SCORE_L2SQ, V>), grid, kThreads, 0, st, e, r, pos_h, pos_r, pos_t, neg_h,     \
+    else OEA_LAUNCH((k_score_margin_weighted<OEA_SCORE_L2SQ, V>), grid, kThreads, 0, st, M, pos_h, pos_r, pos_t, neg_h,     \
                     neg_r, neg_t, n, weights, recip, scale, loss->margin, loss_out)
     OEA_DISPATCH_VEC(ent->pitch, CALL);
 #undef CALL

@@ -1,4 +1,5 @@
 """Builds tests/emu/libemu_oea.so: the product's kernel sources on the CPU warp emulator (test infrastructure)."""
+import glob
 import os
 import subprocess
 
@@ -6,8 +7,11 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(HERE, "libemu_oea.so")
 SRC = os.path.join(HERE, "emu_kernels.cpp")
 CSRC = os.path.join(os.path.dirname(os.path.dirname(HERE)), "openea_b200", "csrc")
-DEPS = [SRC, os.path.join(HERE, "cuda_host_emu.h")] + [os.path.join(CSRC, f) for f in
-                                                        ("oea_triple_ext.cu", "oea_sampler.cu", "oea_optim_ext.cu", "oea_triple_grouped.cu", "oea_triple_weighted.cu", "oea_spmm.cu", "oea_triple.cu", "oea_sim.cu", "oea_pipeline.cu", "oea_match.cu", "oea_p2p.cu", "oea_sampler.cuh", "oea_rowmath.cuh", "oea_common.cuh")]
+DEPS = [SRC, os.path.join(HERE, "cuda_host_emu.h"), os.path.join(os.path.dirname(os.path.dirname(HERE)), "include", "oea.h")] + \
+    [os.path.join(CSRC, f) for f in ("oea_triple_ext.cu", "oea_sampler.cu", "oea_optim_ext.cu", "oea_triple_grouped.cu",
+                                     "oea_triple_weighted.cu", "oea_spmm.cu", "oea_triple.cu", "oea_sim.cu", "oea_pipeline.cu",
+                                     "oea_match.cu", "oea_p2p.cu")] + \
+    sorted(glob.glob(os.path.join(CSRC, "*.cuh")))       # every header: a stale library must not pass
 
 
 def cuda_include():

@@ -86,7 +86,7 @@ def test_emulated_fed_scorers_past_one_wave(cpu_engine, monkeypatch):
     wave = _wave(lib, 8)
     for d, loss_norm, loss, k in ((4, "L2", "limited", 2), (129, "L1", "logistic", 2)):
         n_pos = 1100
-        assert n_pos * (1 + k) > 3 * wave                                         # k_score_fed: a warp per triple
+        assert n_pos * (1 + k) > 3 * wave                                         # oea_triple_score_fed: a warp per triple
         kc.check_fed(e, "cpu", d, loss_norm, loss, k, n_pos=n_pos, hot=0.25, n_ent=400, n_rel=20, seed=d)
     n_pos = 3201
     assert (n_pos + 1) // 2 > 3 * _wave(lib, 4)                                   # k_score_fed_duo: two positives per warp

@@ -66,7 +66,7 @@ def test_fed_scorers_past_three_waves(cuda_device):
     big = dict(hot=0.25, n_ent=20000, n_rel=40, ref_dev=cuda_device)
     for d, loss_norm, loss, k in ((100, "L2", "limited", 2), (129, "L1", "logistic", 2), (512, "L2", "logistic", 1)):
         n_pos = 3 * wave + 7
-        assert n_pos * (1 + k) > 3 * wave                                          # k_score_fed: a warp per triple
+        assert n_pos * (1 + k) > 3 * wave                                          # oea_triple_score_fed: a warp per triple
         kc.check_fed(eng, cuda_device, d, loss_norm, loss, k, n_pos=n_pos, seed=d, **big)
     n_pos = 6 * wave + 1
     assert (n_pos + 1) // 2 > 3 * wave                                             # duo: two positives per warp
