@@ -521,7 +521,8 @@ typedef struct oea_spmm_hubs {
  * gcn_align.py:259-267) or masking by mask_src > 0 (relu backward).  Replaces tf.sparse_tensor_dense_matmul
  * (gcn_align.py:83, alinet.py:581, rdgcn.py:187).  d % 4 == 0, d <= 512.  Rows with at most the threshold run
  * one warp each; hub rows go segment by segment through `workspace` (>= oea_spmm_workspace_bytes(n_seg, d))
- * and are summed in order (deterministic).  hubs may be NULL when no row exceeds the threshold.
+ * and are summed in order (deterministic).  With hubs NULL (or n_long == 0) every row runs one warp each, whatever
+ * its length: correct, but a hub row then sets the kernel's critical path.
  * The backward pass is the same call on the CSR of Aᵀ. */
 int oea_spmm_long_row_threshold(void);
 int oea_spmm_segment_nnz(void);

@@ -10,6 +10,8 @@
 // LONG_ROW non-zeros are handled one warp per row (col/val fetched 32 at a time, coalesced, and
 // broadcast by shuffle; the X row is read with 128-bit loads); hub rows (Zipf degree) get a whole CTA
 // cut into 512-non-zero segments (one CTA each) whose partial rows are added in order — no atomics, deterministic.
+#include <climits>
+
 #include "oea_common.cuh"
 
 namespace oea {
@@ -94,13 +96,14 @@ __device__ __forceinline__ void spmm_store(const Acc<VEC>& acc, float* __restric
 template <int VEC>
 __global__ void __launch_bounds__(SPMM_THREADS)
 k_spmm_warp_rows(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ col, const float* __restrict__ val,
-                 int n_rows, const float* __restrict__ X, int ldx, float* __restrict__ Y, int ldy, int d4, SpmmEpi epi) {
+                 int n_rows, int max_len, const float* __restrict__ X, int ldx, float* __restrict__ Y, int ldy, int d4,
+                 SpmmEpi epi) {
     const int lane = threadIdx.x & 31;
     const int warp_global = blockIdx.x * SPMM_WARPS + (threadIdx.x >> 5);
     const int n_warps = gridDim.x * SPMM_WARPS;
     for (int row = warp_global; row < n_rows; row += n_warps) {
         const int p0 = __ldg(rowptr + row), p1 = __ldg(rowptr + row + 1);
-        if (p1 - p0 > LONG_ROW) continue;   // hub row: k_spmm_segments + k_spmm_finalize
+        if (p1 - p0 > max_len) continue;    // hub row: k_spmm_segments + k_spmm_finalize
         Acc<VEC> acc;
         acc_zero(acc);
         spmm_span<VEC>(col, val, p0, p1, X, ldx, d4, lane, acc);
@@ -254,12 +257,16 @@ extern "C" int oea_spmm_csr(const oea_csr* A, const oea_spmm_hubs* hubs,
     cudaStream_t st = (cudaStream_t)stream;
     SpmmEpi epi{relu, mask_src, beta};
     const int d4 = d >> 2;
+    // with a hub plan the warp-per-row kernel leaves rows of more than LONG_ROW non-zeros to the segment kernels;
+    // without one it takes every row, so no row is left unwritten
+    const int max_len = n_long > 0 ? LONG_ROW : INT_MAX;
     const int blocks = (A->n_rows + SPMM_WARPS - 1) / SPMM_WARPS;
     const int grid = blocks < spmm_sm_count() * 8 ? blocks : spmm_sm_count() * 8;
     float* partial = (float*)workspace;
 #define OEA_SPMM(V)                                                                                                          \
     do {                                                                                                                     \
-        OEA_LAUNCH(k_spmm_warp_rows<V>, grid, SPMM_THREADS, 0, st, A->rowptr, A->col, A->val, A->n_rows, X, ldx, Y, ldy, d4, epi); \
+        OEA_LAUNCH(k_spmm_warp_rows<V>, grid, SPMM_THREADS, 0, st, A->rowptr, A->col, A->val, A->n_rows, max_len,      \
+                   X, ldx, Y, ldy, d4, epi);                                                                                 \
         if (n_long > 0) {                                                                                                    \
             OEA_LAUNCH(k_spmm_segments<V>, n_seg, SPMM_THREADS, SPMM_WARPS * V * 32 * sizeof(float4), st,                    \
                 A->rowptr, A->col, A->val, hubs->long_rows, hubs->seg_row, hubs->seg_start, n_seg, X, ldx, partial, d, d4);  \

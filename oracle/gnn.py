@@ -98,17 +98,30 @@ def reference_alinet_builders():
     return ns
 
 
+def edge_softmax(adj, s1, s2, slope=0.2, edge_logits=None, dtype=None):
+    """alpha [nnz] in the order of sp.coo_matrix(adj) (CSR order for a CSR `adj`): the row softmax of
+    leaky_relu(a_ij (s1_i + s2_j)), or of leaky_relu(edge_logits) when they are given (RDGCN), with torch autograd."""
+    m = sp.coo_matrix(adj)
+    row = torch.as_tensor(m.row, dtype=torch.long)
+    dtype = dtype or (edge_logits if edge_logits is not None else s1).dtype
+    if edge_logits is None:
+        col = torch.as_tensor(m.col, dtype=torch.long)
+        pre = torch.as_tensor(m.data, dtype=dtype) * (s1[row] + s2[col])
+    else:
+        pre = edge_logits
+    logit = torch.nn.functional.leaky_relu(pre, slope)
+    mx = torch.full((m.shape[0],), -1e30, dtype=dtype).scatter_reduce(0, row, logit, "amax")
+    ex = torch.exp(logit - mx[row])
+    den = torch.zeros(m.shape[0], dtype=dtype).index_add(0, row, ex)
+    return ex / den[row]
+
+
 def edge_softmax_aggregate(adj, s1, s2, M, slope=0.2):
     """Σ_j softmax_j(leaky_relu(a_ij (s1_i + s2_j))) M_j over the non-zeros of `adj` (scipy), with torch autograd."""
     m = sp.coo_matrix(adj)
     row = torch.as_tensor(m.row, dtype=torch.long)
     col = torch.as_tensor(m.col, dtype=torch.long)
-    a = torch.as_tensor(m.data, dtype=M.dtype)
-    logit = torch.nn.functional.leaky_relu(a * (s1[row] + s2[col]), slope)
-    mx = torch.full((m.shape[0],), -1e30, dtype=M.dtype).scatter_reduce(0, row, logit, "amax")
-    ex = torch.exp(logit - mx[row])
-    den = torch.zeros(m.shape[0], dtype=M.dtype).index_add(0, row, ex)
-    alpha = ex / den[row]
+    alpha = edge_softmax(m, s1, s2, slope, dtype=M.dtype)
     return torch.zeros(m.shape[0], M.shape[1], dtype=M.dtype).index_add(0, row, alpha[:, None] * M[col])
 
 
