@@ -9,8 +9,8 @@
 // chains are in flight per warp — the kernel is latency/issue bound (dependent gathers per positive over L2-resident
 // tables), not bandwidth bound.  A step of B positives needs B/2 warp tasks, so the
 // 5 000-positive step of the 15K shape fits one resident wave without the 2-tasks-vs-1 tail of the octet kernel.
-// Same maths and — for the sampled source — the same draws as k_score_sampled_oct (modules/base/losses.py:15-73,
-// modules/train/batch.py:36-119, initializers.py:26); requires k <= 16.
+// Same maths as the octet kernel and — for the sampled source — the same draws as every sampled scorer
+// (modules/base/losses.py:15-73, modules/train/batch.py:36-119, initializers.py:26); requires k <= 16.
 //
 // Two sources of (positive, negatives): SAMPLED (fused on-device sampler, oea_sampler.cuh) and FED (index vectors in the
 // reference's batch layout: the k negatives of positive p at p·k … p·k+k−1, batch.py:36-45).  A fed negative that does
@@ -56,13 +56,8 @@ __device__ __forceinline__ float cross_oct_sum(float v) {
     return v;
 }
 
-#ifndef OEA_DUO_WARPS
-#define OEA_DUO_WARPS 4
-#endif
-#ifndef OEA_DUO_MINB
-#define OEA_DUO_MINB 5      // 5 CTAs x 4 warps: at most 96 registers per thread, no spills
-#endif
-constexpr int kDuoWarps = OEA_DUO_WARPS;
+constexpr int kDuoWarps = 4;
+constexpr int kDuoMinB = 5;      // 5 CTAs x 4 warps: at most 96 registers per thread, no spills
 constexpr int kDuoThreads = kDuoWarps * OEA_WARP;
 constexpr int kDuoMaxK = 16;
 
@@ -395,13 +390,6 @@ __device__ __forceinline__ void duo_score_body(const TableDev& ent, const TableD
     const float warp_loss = warp_sum(lane_loss);
     LossAcc acc{s_loss};
     acc.flush(warp_loss, loss_out, kDuoWarps);
-}
-
-// OEA_SCORE_DUO=0 keeps the octet kernels (one positive per warp) for every shape: A/B measurements and tests of both.
-inline bool oea_use_duo(int k) {
-    if (k > kDuoMaxK) return false;
-    const char* v = getenv("OEA_SCORE_DUO");   // read per call: tests flip it inside one process
-    return !(v != nullptr && v[0] == '0');
 }
 
 }  // namespace oea

@@ -11,7 +11,6 @@
 // Work decomposition: one warp per positive + its k negatives (k_score_sampled, oea_transe.cuh), or the octet / duo
 // layouts (8 lanes per row) for the squared-L2 score at pitch <= 128.  The fed scorer (one warp per triple) is
 // oea_triple_score_fed in oea_triple_ext.cu.
-#include <stdlib.h>
 #include "oea_rowmath.cuh"
 #include "oea_rowopt.cuh"
 #include "oea_sampler.cuh"
@@ -42,16 +41,8 @@ k_score_sampled(TableDev ent, TableDev rel, const __grid_constant__ SampledParam
 // negatives: only Σ g_j·ê_j (per corrupted side) and Σ g_j are accumulated per octet, merged across the
 // 4 octets once, and octets 0/1/2 finish rows h / r / t.
 // ------------------------------------------------------------------------------------------------
-#ifndef OEA_OCT_WARPS
-#define OEA_OCT_WARPS 4
-#endif
-#ifndef OEA_OCT_MINB
-#define OEA_OCT_MINB 6       // 6 CTAs × 4 warps: at most 80 registers per thread
-#endif
-#ifndef OEA_OCT_E_SMEM
-#define OEA_OCT_E_SMEM 1
-#endif
-constexpr int kOctWarps = OEA_OCT_WARPS;      // warps per CTA of the octet kernel
+constexpr int kOctWarps = 4;      // warps per CTA of the octet kernel
+constexpr int kOctMinB = 6;       // 6 CTAs × 4 warps: at most 80 registers per thread
 constexpr int kOctThreads = kOctWarps * OEA_WARP;
 
 // Per-warp staging in shared memory.  The kernel is issue-latency bound (≈2 000 warp instructions per positive on
@@ -61,10 +52,8 @@ constexpr int kOctThreads = kOctWarps * OEA_WARP;
 struct OctStage {
     float4 hr[4][8];     // ĥ + r̂   (slot q = l + 8·i)
     float4 rt[4][8];     // r̂ − t̂
-#if OEA_OCT_E_SMEM
     float4 Eh[4][32];    // Σ g_j·ê_j over this lane's octet, head-corrupted negatives
     float4 Et[4][32];    //                                  tail-corrupted
-#endif
 };
 
 __device__ __forceinline__ void oct_score_body(const TableDev& ent, const TableDev& rel, const SampledParams& P,
@@ -133,10 +122,8 @@ __device__ __forceinline__ void oct_score_body(const TableDev& ent, const TableD
                 if (oct == 0) { S.hr[i][l] = hr; S.rt[i][l] = rt; }
                 const float4 up = hr - c;
                 dot4_acc2(sp_part, up, up);
-#if OEA_OCT_E_SMEM
                 S.Eh[i][lane] = f4(0.f);
                 S.Et[i][lane] = f4(0.f);
-#endif
             }
             sp = oct_sum(sp_part.x + sp_part.y);
         }
@@ -146,11 +133,6 @@ __device__ __forceinline__ void oct_score_body(const TableDev& ent, const TableD
         if (lane == 0) lane_loss += Lp;
 
         // ---- phase 2: negatives, four at a time (octet o takes negative 4·round + o) ----
-#if !OEA_OCT_E_SMEM
-        R4 Eh, Et;   // Σ g_j·ê_j over head- / tail-corrupted negatives of this octet
-#pragma unroll
-        for (int i = 0; i < 4; ++i) { Eh.v[i] = f4(0.f); Et.v[i] = f4(0.f); }
-#endif
         float Gh_s = 0.f, Gt_s = 0.f;
         const int rounds = (P.diag & 4) ? 0 : (k + 3) >> 2;
         for (int round = 0; round < rounds; ++round) {
@@ -193,17 +175,11 @@ __device__ __forceinline__ void oct_score_body(const TableDev& ent, const TableD
                 // d s/d ê = ±2u ; through the normaliser: (ĝ − ê<ê,ĝ>)/‖x‖
                 const float c = 2.f * sgn * g * ie;
                 const float proj = (ent.norm && sse >= kNormEps) ? de : 0.f;
-#if OEA_OCT_E_SMEM
                 float4* acc = head ? &S.Eh[0][0] : &S.Et[0][0];
-#endif
                 float* grow = ent.g + (size_t)e_id * ent.pitch;
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
-#if OEA_OCT_E_SMEM
                     acc[i * 32 + lane] = fma4(e.v[i], g, acc[i * 32 + lane]);
-#else
-                    if (head) Eh.v[i] = fma4(e.v[i], g, Eh.v[i]); else Et.v[i] = fma4(e.v[i], g, Et.v[i]);
-#endif
                     if (!(P.diag & 2) && l + 8 * i < p4) red_add4(grow + 4 * (l + 8 * i), fma4(e.v[i], -proj, u.v[i]) * c);
                 }
                 if (head) Gh_s += g; else Gt_s += g;
@@ -235,14 +211,8 @@ __device__ __forceinline__ void oct_score_body(const TableDev& ent, const TableD
             float2 dpart2 = make_float2(0.f, 0.f);
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-#if OEA_OCT_E_SMEM
                 const float4 eh = (S.Eh[i][l] + S.Eh[i][8 + l]) + (S.Eh[i][16 + l] + S.Eh[i][24 + l]);
                 const float4 et = (S.Et[i][l] + S.Et[i][8 + l]) + (S.Et[i][16 + l] + S.Et[i][24 + l]);
-#else
-                float4 eh = Eh.v[i], et = Et.v[i];
-                eh.x = cross_oct_sum(eh.x); eh.y = cross_oct_sum(eh.y); eh.z = cross_oct_sum(eh.z); eh.w = cross_oct_sum(eh.w);
-                et.x = cross_oct_sum(et.x); et.y = cross_oct_sum(et.y); et.z = cross_oct_sum(et.z); et.w = cross_oct_sum(et.w);
-#endif
                 // α(hr − t̂) + β(G_t·hr − E_t) + γ(G_h·rt + E_h)
                 float4 g4 = S.hr[i][l] * c_hr;
                 g4 = fma4(S.rt[i][l], c_rt, g4);
@@ -268,7 +238,7 @@ __device__ __forceinline__ void oct_score_body(const TableDev& ent, const TableD
     acc.flush(warp_loss, loss_out, kOctWarps);
 }
 
-__global__ void __launch_bounds__(kOctThreads, OEA_OCT_MINB)
+__global__ void __launch_bounds__(kOctThreads, kOctMinB)
 k_score_sampled_oct(TableDev ent, TableDev rel, const __grid_constant__ SampledParams P, oea_loss_cfg cfg,
                     double* __restrict__ loss_out, int32_t* __restrict__ dbg) {
     __shared__ double s_loss[kOctWarps];
@@ -280,7 +250,7 @@ k_score_sampled_oct(TableDev ent, TableDev rel, const __grid_constant__ SampledP
 // Saves the second launch and its ramp; the grid is one resident wave by
 // construction (grid_one_wave), which is what a cooperative launch requires.
 template <int KIND>
-__global__ void __launch_bounds__(kOctThreads, OEA_OCT_MINB)
+__global__ void __launch_bounds__(kOctThreads, kOctMinB)
 k_step_sampled_oct(TableDev ent, TableDev rel, const __grid_constant__ SampledParams P, oea_loss_cfg cfg,
                    double* __restrict__ loss_out, OptTab A, OptTab B, float lr) {
     __shared__ double s_loss[kOctWarps];
@@ -291,7 +261,7 @@ k_step_sampled_oct(TableDev ent, TableDev rel, const __grid_constant__ SampledPa
 }
 
 // The duo scorer (oea_duo.cuh): two positives per warp, sampled source.
-__global__ void __launch_bounds__(kDuoThreads, OEA_DUO_MINB)
+__global__ void __launch_bounds__(kDuoThreads, kDuoMinB)
 k_score_sampled_duo(TableDev ent, TableDev rel, const __grid_constant__ SampledParams P, oea_loss_cfg cfg,
                     double* __restrict__ loss_out, int32_t* __restrict__ dbg) {
     __shared__ double s_loss[kDuoWarps];
@@ -302,7 +272,7 @@ k_score_sampled_duo(TableDev ent, TableDev rel, const __grid_constant__ SampledP
 
 // The whole sampled training step as ONE cooperative launch, duo scorer: score + gradients, grid barrier, row optimiser.
 template <int KIND>
-__global__ void __launch_bounds__(kDuoThreads, OEA_DUO_MINB)
+__global__ void __launch_bounds__(kDuoThreads, kDuoMinB)
 k_step_sampled_duo(TableDev ent, TableDev rel, const __grid_constant__ SampledParams P, oea_loss_cfg cfg,
                    double* __restrict__ loss_out, OptTab A, OptTab B, float lr) {
     __shared__ double s_loss[kDuoWarps];
@@ -432,18 +402,6 @@ extern "C" int oea_rowopt_apply(const oea_table* t, const oea_opt_cfg* opt, void
     return OEA_OK;
 }
 
-// OEA_SCORE_V1=1 selects the warp-per-row kernel for every shape (A/B measurements, tests of both paths).
-static bool oea_force_v1() {
-    const char* v = getenv("OEA_SCORE_V1");   // read per call: tests flip it inside one process
-    return v != nullptr && v[0] == '1';
-}
-
-// OEA_NO_FUSE=1 keeps the sampled step as two launches (score, optimiser): A/B of the cooperative fused launch.
-static bool oea_no_fuse() {
-    const char* v = getenv("OEA_NO_FUSE");
-    return v != nullptr && v[0] == '1';
-}
-
 // Argument checks + step parameters shared by the score-only and the fused-step entry points.
 static int sampled_prepare(const oea_table* ent, const oea_table* rel, const oea_kg_view* kg1, const oea_kg_view* kg2,
                            const oea_tripleset* tset, const oea_sample_cfg* smp, const oea_loss_cfg* loss,
@@ -473,23 +431,29 @@ extern "C" int oea_triple_score_sampled(const oea_table* ent, const oea_table* r
     if (n_pos_out) OEA_CUDA_TRY(cudaMemcpyAsync(n_pos_out, &n_pos, sizeof(int), cudaMemcpyHostToDevice, st));
     if (n_pos == 0) return OEA_OK;
     TableDev e = table_dev(ent), r = table_dev(rel);
-    const bool l1 = loss->score_kind == OEA_SCORE_L1;
-    if (!l1 && ent->pitch <= 128 && !oea_force_v1() && oea_use_duo(P.k)) {
-        const int pairs = ((n_pos + P.shard_world - 1) / P.shard_world + 1) / 2;
-        const int grid = grid_one_wave<k_score_sampled_duo>(pairs, kDuoWarps);
+    const int n_mine = (n_pos + P.shard_world - 1) / P.shard_world;
+#define CALL(SCORE, V)                                                                                     \
+    do { const int grid = grid_one_wave<k_score_sampled<SCORE, V>>(n_mine);                                \
+         OEA_LAUNCH((k_score_sampled<SCORE, V>), grid, kThreads, 0, st, e, r, P, *loss, loss_out, dbg_neg); } while (0)
+#define CALL_L1(V) CALL(OEA_SCORE_L1, V)
+    // Squared L2: the octet layouts up to pitch 128 (duo at k <= 16, octet above), warp per positive past it
+    if (loss->score_kind == OEA_SCORE_L1) {
+        OEA_DISPATCH_VEC(ent->pitch, CALL_L1);
+    } else if (ent->pitch <= 128 && P.k <= kDuoMaxK) {
+        const int grid = grid_one_wave<k_score_sampled_duo>((n_mine + 1) / 2, kDuoWarps);
         OEA_LAUNCH(k_score_sampled_duo, grid, kDuoThreads, 0, st, e, r, P, *loss, loss_out, dbg_neg);
-    } else if (!l1 && ent->pitch <= 128 && !oea_force_v1()) {
-        const int grid = grid_one_wave<k_score_sampled_oct>((n_pos + P.shard_world - 1) / P.shard_world, kOctWarps);
+    } else if (ent->pitch <= 128) {
+        const int grid = grid_one_wave<k_score_sampled_oct>(n_mine, kOctWarps);
         OEA_LAUNCH(k_score_sampled_oct, grid, kOctThreads, 0, st, e, r, P, *loss, loss_out, dbg_neg);
+    } else if (ent->pitch <= 256) {
+        CALL(OEA_SCORE_L2SQ, 2);
+    } else if (ent->pitch <= 384) {
+        CALL(OEA_SCORE_L2SQ, 3);
     } else {
-#define CALL(V)                                                                                              \
-    if (l1) { const int grid = grid_one_wave<k_score_sampled<OEA_SCORE_L1, V>>((n_pos + P.shard_world - 1) / P.shard_world);                     \
-              OEA_LAUNCH((k_score_sampled<OEA_SCORE_L1, V>), grid, kThreads, 0, st, e, r, P, *loss, loss_out, dbg_neg); } \
-    else { const int grid = grid_one_wave<k_score_sampled<OEA_SCORE_L2SQ, V>>((n_pos + P.shard_world - 1) / P.shard_world);                      \
-           OEA_LAUNCH((k_score_sampled<OEA_SCORE_L2SQ, V>), grid, kThreads, 0, st, e, r, P, *loss, loss_out, dbg_neg); }
-        OEA_DISPATCH_VEC(ent->pitch, CALL);
-#undef CALL
+        CALL(OEA_SCORE_L2SQ, 4);
     }
+#undef CALL_L1
+#undef CALL
     OEA_LAUNCH_CHECK();
     return OEA_OK;
 }
@@ -777,9 +741,9 @@ extern "C" int oea_triple_step_sampled(const oea_table* ent, const oea_table* re
                                        double* loss_out, int32_t* n_pos_out, void* stream) {
     if (!opt) return OEA_ERR_NULL;
     if (smp && smp->shard_world > 1) return OEA_ERR_RANGE;   // sharded batches: score_sampled → gradient exchange → rowopt
-    // One cooperative launch when the octet kernel applies and the optimiser is row-sparse (Adagrad / SGD)
-    const bool fuse = loss && ent && rel && loss->score_kind == OEA_SCORE_L2SQ && ent->pitch <= 128 && !oea_force_v1() &&
-                      (opt->kind == OEA_OPT_ADAGRAD || opt->kind == OEA_OPT_SGD) && !oea_no_fuse();
+    // One cooperative launch when an octet-layout kernel applies and the optimiser is row-sparse (Adagrad / SGD)
+    const bool fuse = loss && ent && rel && loss->score_kind == OEA_SCORE_L2SQ && ent->pitch <= 128 &&
+                      (opt->kind == OEA_OPT_ADAGRAD || opt->kind == OEA_OPT_SGD);
     if (!fuse) {
         int rc = oea_triple_score_sampled(ent, rel, kg1, kg2, tset, smp, loss, loss_out, n_pos_out, nullptr, stream);
         if (rc) return rc;
@@ -797,7 +761,7 @@ extern "C" int oea_triple_step_sampled(const oea_table* ent, const oea_table* re
     OptTab A{ent->weight, ent->grad, ent->state1, ent->touched, ent->rows}, B{rel->weight, rel->grad, rel->state1, rel->touched, rel->rows};
     oea_loss_cfg cfg = *loss;
     float lr = opt->lr;
-    if (oea_use_duo(P.k)) {
+    if (P.k <= kDuoMaxK) {
         const int pairs = (n_pos + 1) / 2;
         if (opt->kind == OEA_OPT_ADAGRAD) {
             const int grid = grid_one_wave<k_step_sampled_duo<OEA_OPT_ADAGRAD>>(pairs, kDuoWarps);

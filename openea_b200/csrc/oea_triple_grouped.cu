@@ -7,7 +7,6 @@
 //
 // Opt-in: oea_triple_step_fed_host uses it when OEA_FED_GROUPED=1 (until it has been timed on hardware);
 // tests/test_emu_triple_grouped.py checks it on the CPU warp emulator against the C oracle.
-#include <stdlib.h>
 #include <cooperative_groups.h>
 
 #include "oea_rowmath.cuh"
@@ -46,7 +45,7 @@ k_step_fed_grouped(TableDev ent, TableDev rel, FedBatch F, oea_loss_cfg cfg, dou
 
 // The duo scorer (oea_duo.cuh) on a fed batch: two positives per warp, octet row layout, squared-L2 score, pitch <= 128,
 // k <= 16.  Negatives that share fewer than two rows with their positive take the general-triple path inside the body.
-__global__ void __launch_bounds__(kDuoThreads, OEA_DUO_MINB)
+__global__ void __launch_bounds__(kDuoThreads, kDuoMinB)
 k_score_fed_duo(TableDev ent, TableDev rel, FedBatch F, oea_loss_cfg cfg, double* __restrict__ loss_out) {
     __shared__ double s_loss[kDuoWarps];
     __shared__ DuoStage s_stage[kDuoWarps];
@@ -55,7 +54,7 @@ k_score_fed_duo(TableDev ent, TableDev rel, FedBatch F, oea_loss_cfg cfg, double
 }
 
 template <int KIND>
-__global__ void __launch_bounds__(kDuoThreads, OEA_DUO_MINB)
+__global__ void __launch_bounds__(kDuoThreads, kDuoMinB)
 k_step_fed_duo(TableDev ent, TableDev rel, FedBatch F, oea_loss_cfg cfg, double* __restrict__ loss_out, OptTab A, OptTab B, float lr) {
     __shared__ double s_loss[kDuoWarps];
     __shared__ DuoStage s_stage[kDuoWarps];
@@ -87,7 +86,7 @@ extern "C" int oea_triple_score_fed_grouped(const oea_table* ent, const oea_tabl
     TableDev e = table_dev(ent), r = table_dev(rel);
     const bool l1 = loss->score_kind == OEA_SCORE_L1;
     const FedBatch F{pos_h, pos_r, pos_t, neg_h, neg_r, neg_t, n_pos, k};
-    if (!l1 && ent->pitch <= 128 && oea_use_duo(k)) {
+    if (!l1 && ent->pitch <= 128 && k <= kDuoMaxK) {
         const int grid = grid_one_wave<k_score_fed_duo>((n_pos + 1) / 2, kDuoWarps);
         OEA_LAUNCH(k_score_fed_duo, grid, kDuoThreads, 0, (cudaStream_t)stream, e, r, F, *loss, loss_out);
         OEA_LAUNCH_CHECK();
@@ -131,7 +130,7 @@ extern "C" int oea_triple_step_fed_grouped(const oea_table* ent, const oea_table
     oea_loss_cfg cfg = *loss;
     float lr = opt->lr;
     FedBatch F{pos_h, pos_r, pos_t, neg_h, neg_r, neg_t, n_pos, k};
-    if (ent->pitch <= 128 && oea_use_duo(k)) {
+    if (ent->pitch <= 128 && k <= kDuoMaxK) {
         if (opt->kind == OEA_OPT_ADAGRAD) {
             const int grid = grid_one_wave<k_step_fed_duo<OEA_OPT_ADAGRAD>>((n_pos + 1) / 2, kDuoWarps);
             OEA_CUDA_TRY(OEA_LAUNCH_COOPERATIVE(k_step_fed_duo<OEA_OPT_ADAGRAD>, grid, kDuoThreads, st, e, r, F, cfg, loss_out, A, B, lr));

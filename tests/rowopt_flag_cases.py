@@ -123,12 +123,12 @@ def fed_batch(rng, n_ent, n_rel, n_pos, k=3):
     return pos, np.ascontiguousarray(neg)
 
 
-def run_fed_step(eng, trainer, pattern, dim, opt, device, base_a, base_b, seed, n_pos):
+def run_fed_step(eng, trainer, pattern, dim, opt, device, base_a, base_b, seed, n_pos, k=3):
     """The one-launch fed step on a placed trainer, checked against the optimiser restatement applied to what the
     two-launch scorer leaves on a second trainer with the same placed state (the scorers' float atomics order their
     sums differently, hence the suite's looser tolerances on the flagged rows)."""
     ref, _ = place(eng, np.random.default_rng(seed), pattern, dim, opt, device, base_a, base_b)
-    pos, neg = fed_batch(np.random.default_rng(seed + 1), trainer.ent.rows, trainer.rel.rows, n_pos)
+    pos, neg = fed_batch(np.random.default_rng(seed + 1), trainer.ent.rows, trainer.rel.rows, n_pos, k)
     pos_t, neg_t = torch.from_numpy(pos).to(device), torch.from_numpy(neg).to(device)
     ref.score_fed(pos_t, neg_t, grouped=True)
     start = {"ent": snapshot(ref.ent), "rel": snapshot(ref.rel)}

@@ -27,8 +27,6 @@ def cpu_engine(monkeypatch):
             fn.restype, fn.argtypes = res, args
     monkeypatch.setattr(L, "load", lambda: lib)
     monkeypatch.setattr(eng, "_stream_ptr", lambda: C.c_void_p(0))
-    for var in ("OEA_NO_FUSE", "OEA_SCORE_V1", "OEA_SCORE_DUO"):
-        monkeypatch.delenv(var, raising=False)
     return eng, lib
 
 
@@ -43,17 +41,16 @@ def _wave(lib, warps_per_block):
 
 @pytest.mark.parametrize("loss_norm", ["L2", "L1"])
 @pytest.mark.parametrize("d", kc.DIMS)
-def test_emulated_fed_scorers_at_every_width(cpu_engine, monkeypatch, d, loss_norm):
-    """oea_triple_score_fed and oea_triple_score_fed_grouped (duo at pitch <= 128 for L2, the warp-per-positive kernel
-    otherwise and with OEA_SCORE_DUO=0), all five losses, edge rows in every batch."""
+def test_emulated_fed_scorers_at_every_width(cpu_engine, d, loss_norm):
+    """oea_triple_score_fed and oea_triple_score_fed_grouped (duo at pitch <= 128 for L2 and k <= 16, the
+    warp-per-positive kernel otherwise: at L2 and pitch <= 128 with k = 17), all five losses, edge rows in every batch."""
     e, _ = cpu_engine
     for loss, k in kc.LOSSES:
         kc.check_fed(e, "cpu", d, loss_norm, loss, k, seed=d + k)
         kc.check_fed(e, "cpu", d, loss_norm, loss, k, seed=d + k, grouped=True)
-        if loss_norm == "L2" and d <= 128:
-            monkeypatch.setenv("OEA_SCORE_DUO", "0")
-            kc.check_fed(e, "cpu", d, loss_norm, loss, k, seed=d + k, grouped=True)
-            monkeypatch.delenv("OEA_SCORE_DUO")
+    if loss_norm == "L2" and d <= 128:
+        for loss in ("limited", "logistic"):
+            kc.check_fed(e, "cpu", d, loss_norm, loss, 17, seed=d + 17, grouped=True)
     # unnormalised tables scaled so that the scores reach ~100: softplus / sigmoid far from 0
     scale = 6.0 if loss_norm == "L2" else 70.0 / np.sqrt(d)
     for loss, k in (("logistic", 2), ("logsigmoid", 0)):
@@ -79,7 +76,7 @@ def test_emulated_duo_scorers_take_the_unpaired_last_positive(cpu_engine, d, n_p
         kc.check_sampled(e, "cpu", d, "L2", "limited", 5, n_pos, seed=n_pos)
 
 
-def test_emulated_fed_scorers_past_one_wave(cpu_engine, monkeypatch):
+def test_emulated_fed_scorers_past_one_wave(cpu_engine):
     """Three waves and more: the grid-stride loops' later iterations, the duo kernel's per-warp staging reused across
     them and the loss carried in fp32 across iterations; one entity in a quarter of the triples."""
     e, lib = cpu_engine
@@ -96,13 +93,12 @@ def test_emulated_fed_scorers_past_one_wave(cpu_engine, monkeypatch):
     kc.check_fed(e, "cpu", 4, "L1", "margin-based", 1, n_pos=n_pos, grouped=True, hot=0.25, n_ent=2000, n_rel=20, seed=6)
 
 
-def test_emulated_sampled_scorers_past_one_wave(cpu_engine, monkeypatch):
+def test_emulated_sampled_scorers_past_one_wave(cpu_engine):
     e, lib = cpu_engine
     m = kc.check_sampled(e, "cpu", 12, "L2", "limited", 2, 3300, n_tri=7000, n=900, seed=1)        # duo
     assert (m + 1) // 2 > 3 * _wave(lib, 4)
     m = kc.check_sampled(e, "cpu", 12, "L2", "limited", 20, 1700, n_tri=4000, n=900, seed=2)       # octet: k > 16
     assert m > 3 * _wave(lib, 4)
-    monkeypatch.setenv("OEA_SCORE_V1", "1")
     m = kc.check_sampled(e, "cpu", 129, "L1", "limited", 2, 3300, n_tri=7000, n=900, seed=3)       # warp per positive
     assert m > 3 * _wave(lib, 8)
 
@@ -116,15 +112,13 @@ def test_emulated_one_launch_fed_step_equals_dense_steps(cpu_engine, d, opt):
 
 @pytest.mark.parametrize("variant,d,loss_norm,loss,k", [
     ("duo", 1, "L2", "limited", 6), ("duo", 4, "L2", "margin-based", 1), ("duo", 127, "L2", "logistic", 3),
-    ("duo", 128, "L2", "limited", 16), ("oct", 3, "L2", "limited", 20), ("oct", 128, "L2", "logistic", 4),
+    ("duo", 128, "L2", "limited", 16), ("oct", 3, "L2", "limited", 20), ("oct", 128, "L2", "logistic", 17),
     ("v1", 129, "L1", "limited", 3), ("v1", 256, "L2", "logistic", 2), ("v1", 257, "L1", "margin-based", 1),
     ("v1", 384, "L2", "limited", 3), ("v1", 385, "L1", "logistic", 2), ("v1", 512, "L1", "limited", 3),
     ("v1", 512, "L2", "positive", 0)])
-def test_emulated_sampled_scorers_replay_through_the_reference(cpu_engine, monkeypatch, variant, d, loss_norm, loss, k):
-    """The sampled kernels' debug dump, decoded, scored by the float64 reference: same loss and gradients."""
-    monkeypatch.setenv("OEA_SCORE_DUO", "0" if variant == "oct" else "1")
-    if variant == "v1":
-        monkeypatch.setenv("OEA_SCORE_V1", "1")
+def test_emulated_sampled_scorers_replay_through_the_reference(cpu_engine, variant, d, loss_norm, loss, k):
+    """The sampled kernels' debug dump, decoded, scored by the float64 reference: same loss and gradients.  `variant`
+    names the kernel the shape reaches: duo, oct or v1 (k_score_sampled, one warp per positive)."""
     kc.check_sampled(cpu_engine[0], "cpu", d, loss_norm, loss, k, 33, seed=d + k)
 
 

@@ -44,14 +44,13 @@ def test_emulated_pair_optimiser_updates_exactly_the_flagged_rows(emu_engine, pa
     check_update(trainer, expect_update(before, opt, LR))
 
 
-@pytest.mark.parametrize("duo", ["1", "0"])
+@pytest.mark.parametrize("k", [3, 17])
 @pytest.mark.parametrize("opt", ["Adagrad", "SGD"])
 @pytest.mark.parametrize("dim", DIMS)
 @pytest.mark.parametrize("pattern", sorted(PATTERNS))
-def test_emulated_one_launch_fed_step_updates_placed_and_batch_rows(emu_engine, monkeypatch, pattern, dim, opt, duo):
-    """k_step_fed_duo (OEA_SCORE_DUO=1) and k_step_fed_grouped (0): the placed rows are updated together with the rows
+def test_emulated_one_launch_fed_step_updates_placed_and_batch_rows(emu_engine, pattern, dim, opt, k):
+    """k_step_fed_duo (k <= 16) and k_step_fed_grouped (k = 17): the placed rows are updated together with the rows
     the step's own batch flags."""
-    monkeypatch.setenv("OEA_SCORE_DUO", duo)
-    seed = seed_of(pattern, dim, opt, duo)
+    seed = seed_of(pattern, dim, opt, k)
     trainer, _ = place(emu_engine, np.random.default_rng(seed), pattern, dim, opt, "cpu", BASE_A, BASE_B)
-    run_fed_step(emu_engine, trainer, pattern, dim, opt, "cpu", BASE_A, BASE_B, seed, n_pos=24)
+    run_fed_step(emu_engine, trainer, pattern, dim, opt, "cpu", BASE_A, BASE_B, seed, n_pos=24, k=k)

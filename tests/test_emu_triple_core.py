@@ -14,6 +14,7 @@ from openea_b200 import lib as L
 from oracle import triple as orc
 from tests.emu import build_emu
 from tests.helpers import make_batch, make_tables
+from tests.kernel_edge_cases import decode_dbg
 
 
 @pytest.fixture()
@@ -28,8 +29,6 @@ def cpu_engine(monkeypatch):
             fn.restype, fn.argtypes = res, args
     monkeypatch.setattr(L, "load", lambda: lib)
     monkeypatch.setattr(eng, "_stream_ptr", lambda: C.c_void_p(0))
-    monkeypatch.setenv("OEA_NO_FUSE", "1")            # the one-launch step needs a grid barrier
-    monkeypatch.setenv("OEA_SCORE_V1", "1")           # the warp-per-positive sampled kernel
     return eng
 
 
@@ -96,8 +95,9 @@ def test_emulated_lookup_scatter_and_tensor_level_losses(cpu_engine):
 
 
 def test_emulated_triple_set_and_sampled_scorer_replay(cpu_engine):
-    """oea_tripleset_build + the warp-per-positive sampled kernel: its debug dump, replayed through the fed scorer, gives
-    the same loss and gradients (the check tests/test_triple_gpu.py makes on the GPU)."""
+    """oea_tripleset_build + the sampled kernels at d = 12 (the duo for L2, the warp-per-positive kernel for L1): the
+    debug dump, replayed through the fed scorer, gives the same loss and gradients (the check tests/test_triple_gpu.py
+    makes on the GPU)."""
     rng = np.random.default_rng(8)
     n, n_rel, d = 50, 4, 12
     def kg(lo):
@@ -111,26 +111,21 @@ def test_emulated_triple_set_and_sampled_scorer_replay(cpu_engine):
     from tests.test_emu_sampler import build_tripleset
     want_slots, _ = build_tripleset(np.concatenate([t1, t2]), tset.ent_bits, tset.rel_bits, capacity=tset.capacity)
     assert set(tset.slots.numpy().view(np.uint64).tolist()) == set(want_slots.tolist())       # same keys (probe order may differ)
-    cfg = cpu_engine.loss_cfg("limited", "L2", 0.1, 2.0, 0.2)
     B, k = 32, 3
-    a = cpu_engine.TripleTrainer(cpu_engine.EmbeddingTable(ent, True, device="cpu"),
-                                 cpu_engine.EmbeddingTable(rel, True, device="cpu"), cfg, 0.01)
-    dbg = torch.zeros(B, 2 + k, dtype=torch.int32)
-    n_pos = torch.zeros(1, dtype=torch.int32)
-    a.score_sampled(kg1, kg2, tset, B, k, 1, 4242, dbg=dbg, n_pos_out=n_pos)
-    m = int(n_pos)
-    rows = dbg.numpy()[:m]
-    pos = np.stack([(t2[r[0] - (1 << 30)] if r[0] >= (1 << 30) else t1[r[0]]) for r in rows], 1).astype(np.int32)
-    neg = np.repeat(pos, k, axis=1)
-    for i, r in enumerate(rows):
-        for j in range(k):
-            neg[0 if (r[1] >> j) & 1 else 2, i * k + j] = r[2 + j]
-    b = cpu_engine.TripleTrainer(cpu_engine.EmbeddingTable(ent, True, device="cpu"),
-                                 cpu_engine.EmbeddingTable(rel, True, device="cpu"), cfg, 0.01)
-    b.score_fed(_t(pos), _t(neg))
-    assert a.read_loss() == pytest.approx(b.read_loss(), rel=1e-5)
-    np.testing.assert_allclose(a.ent.grad.numpy(), b.ent.grad.numpy(), rtol=1e-4, atol=1e-6)
-    np.testing.assert_allclose(a.rel.grad.numpy(), b.rel.grad.numpy(), rtol=1e-4, atol=1e-6)
+    for loss_norm in ("L2", "L1"):
+        cfg = cpu_engine.loss_cfg("limited", loss_norm, 0.1, 2.0, 0.2)
+        make = lambda: cpu_engine.TripleTrainer(cpu_engine.EmbeddingTable(ent, True, device="cpu"),
+                                                cpu_engine.EmbeddingTable(rel, True, device="cpu"), cfg, 0.01)
+        a = make()
+        dbg = torch.zeros(B, 2 + k, dtype=torch.int32)
+        n_pos = torch.zeros(1, dtype=torch.int32)
+        a.score_sampled(kg1, kg2, tset, B, k, 1, 4242, dbg=dbg, n_pos_out=n_pos)
+        pos, neg = decode_dbg(dbg.numpy()[:int(n_pos)], t1, t2, k)
+        b = make()
+        b.score_fed(_t(pos), _t(neg))
+        assert a.read_loss() == pytest.approx(b.read_loss(), rel=1e-5), loss_norm
+        np.testing.assert_allclose(a.ent.grad.numpy(), b.ent.grad.numpy(), rtol=1e-4, atol=1e-6, err_msg=loss_norm)
+        np.testing.assert_allclose(a.rel.grad.numpy(), b.rel.grad.numpy(), rtol=1e-4, atol=1e-6, err_msg=loss_norm)
 
 
 def _normed(x, on):
@@ -215,45 +210,44 @@ def test_emulated_pair_distance_loss_matches_autograd(cpu_engine, norm, d, weigh
 
 
 @pytest.fixture(params=["duo", "oct"])
-def cpu_engine_oct(cpu_engine, monkeypatch, request):
-    """The same engine with the octet-layout kernels enabled: the sampled scorer (duo: two positives per warp, the default;
-    oct: one positive per warp, OEA_SCORE_DUO=0) and the one-launch step (score, grid barrier, octet row optimiser —
-    launched as one block on the emulator, so its grid barrier is the block's)."""
-    monkeypatch.delenv("OEA_NO_FUSE")
-    monkeypatch.delenv("OEA_SCORE_V1")
-    monkeypatch.setenv("OEA_SCORE_DUO", "1" if request.param == "duo" else "0")
-    return cpu_engine
+def octet_k(request):
+    """Negatives per positive that reach each octet-layout kernel at squared L2, pitch <= 128: the duo (two positives
+    per warp) takes k <= 16, the octet (one positive per warp) k = 17 … 32.  The one-launch step is launched as one
+    block on the emulator, so its grid barrier is the block's."""
+    return {"duo": 6, "oct": 20}[request.param]
 
 
-def test_emulated_duo_and_octet_scorers_sample_the_same_batch(cpu_engine, monkeypatch):
-    """The duo scorer (two positives per warp) draws, negative for negative, the batch the one-positive octet scorer draws
-    from the same seed, and accumulates the same gradients: odd and even numbers of positives, k = 0 / 1 (margin) / 6 / 16,
-    sharded launches included."""
-    monkeypatch.delenv("OEA_NO_FUSE")
-    monkeypatch.delenv("OEA_SCORE_V1")
+def test_emulated_duo_and_octet_scorers_sample_the_same_batch(cpu_engine):
+    """Every sampled kernel draws the same batch from the same seed (the sampler does not read the score kind): the
+    debug dump of the squared-L2 kernel (the duo, or the octet at k = 20) equals that of the warp-per-positive kernel at
+    L1, and each kernel's loss, gradients and row flags equal the fed scorer's on its decoded dump.  Odd and even
+    numbers of positives, k = 0 / 1 (margin) / 6 / 16 / 20, sharded launches included."""
     rng = np.random.default_rng(77)
     t1, t2, kg1, kg2, tset, _ = _sampled_setup(cpu_engine, rng)
     n, n_rel, d = 50, 4, 12
     ent, rel = make_tables(rng, 2 * n, n_rel, d)
     for loss, k, B, shard in (("limited", 6, 33, None), ("limited", 16, 32, None), ("margin-based", 1, 31, None),
-                              ("positive", 0, 20, None), ("limited", 5, 37, (1, 3)), ("logistic", 3, 34, (0, 2))):
-        got = {}
-        for variant in ("1", "0"):
-            monkeypatch.setenv("OEA_SCORE_DUO", variant)
-            tr = cpu_engine.TripleTrainer(cpu_engine.EmbeddingTable(ent, True, "Adagrad", device="cpu"),
-                                          cpu_engine.EmbeddingTable(rel, True, "Adagrad", device="cpu"),
-                                          cpu_engine.loss_cfg(loss, "L2", 0.8 if loss == "margin-based" else 0.1, 2.0, 0.2), 0.01)
+                              ("positive", 0, 20, None), ("limited", 5, 37, (1, 3)), ("logistic", 3, 34, (0, 2)),
+                              ("limited", 20, 35, None)):
+        dumps = []
+        for loss_norm in ("L2", "L1"):
+            cfg = cpu_engine.loss_cfg(loss, loss_norm, 0.8 if loss == "margin-based" else 0.1, 2.0, 0.2)
+            make = lambda: cpu_engine.TripleTrainer(cpu_engine.EmbeddingTable(ent, True, "Adagrad", device="cpu"),
+                                                    cpu_engine.EmbeddingTable(rel, True, "Adagrad", device="cpu"), cfg, 0.01)
+            tr, ref = make(), make()
             dbg = torch.full((B, 2 + k), -7, dtype=torch.int32)
             tr.score_sampled(kg1, kg2, tset, B, k, 1, 991, dbg=dbg, shard=shard)
-            got[variant] = (dbg.numpy().copy(), tr.ent.grad.numpy().copy(), tr.rel.grad.numpy().copy(),
-                            tr.ent.touched.numpy().copy(), tr.read_loss())
-        a, b = got["1"], got["0"]
-        assert np.array_equal(a[0], b[0]), (loss, k, B, shard)
-        assert (a[0][:, 0] != -7).sum() > 0
-        np.testing.assert_allclose(a[1], b[1], rtol=1e-4, atol=1e-6)
-        np.testing.assert_allclose(a[2], b[2], rtol=1e-4, atol=1e-6)
-        assert np.array_equal(a[3] != 0, b[3] != 0)
-        assert a[4] == pytest.approx(b[4], rel=1e-5)
+            dumps.append(dbg.numpy().copy())
+            live = dumps[-1][:, 0] != -7
+            assert live.sum() > 0
+            pos, neg = decode_dbg(dumps[-1][live], t1, t2, k)
+            ref.score_fed(_t(pos), None if neg is None else _t(neg))
+            what = (loss, loss_norm, k, B, shard)
+            assert tr.read_loss() == pytest.approx(ref.read_loss(), rel=1e-5), what
+            np.testing.assert_allclose(tr.ent.grad.numpy(), ref.ent.grad.numpy(), rtol=1e-4, atol=1e-6, err_msg=str(what))
+            np.testing.assert_allclose(tr.rel.grad.numpy(), ref.rel.grad.numpy(), rtol=1e-4, atol=1e-6, err_msg=str(what))
+            assert np.array_equal(tr.ent.touched.numpy() != 0, ref.ent.touched.numpy() != 0), what
+        assert np.array_equal(dumps[0], dumps[1]), (loss, k, B, shard)
 
 
 def _sampled_setup(engine, rng, opt="Adagrad"):
@@ -272,22 +266,17 @@ def _sampled_setup(engine, rng, opt="Adagrad"):
     return t1, t2, kg1, kg2, tset, make
 
 
-def test_emulated_octet_scorer_replays_through_the_fed_scorer(cpu_engine_oct):
-    """k_score_sampled_oct (four negatives per warp pass, shared rows staged in shared memory): its debug dump replayed
-    through the per-triple fed scorer gives the same loss and gradients."""
+def test_emulated_octet_scorer_replays_through_the_fed_scorer(cpu_engine, octet_k):
+    """k_score_sampled_oct (four negatives per warp pass, shared rows staged in shared memory) and the duo: the debug
+    dump replayed through the per-triple fed scorer gives the same loss and gradients."""
     rng = np.random.default_rng(18)
-    t1, t2, kg1, kg2, tset, make = _sampled_setup(cpu_engine_oct, rng)
-    B, k = 32, 6
+    t1, t2, kg1, kg2, tset, make = _sampled_setup(cpu_engine, rng)
+    B, k = 32, octet_k
     a = make()
     dbg = torch.zeros(B, 2 + k, dtype=torch.int32)
     n_pos = torch.zeros(1, dtype=torch.int32)
     a.score_sampled(kg1, kg2, tset, B, k, 1, 4242, dbg=dbg, n_pos_out=n_pos)
-    rows = dbg.numpy()[:int(n_pos)]
-    pos = np.stack([(t2[r[0] - (1 << 30)] if r[0] >= (1 << 30) else t1[r[0]]) for r in rows], 1).astype(np.int32)
-    neg = np.repeat(pos, k, axis=1)
-    for i, r in enumerate(rows):
-        for j in range(k):
-            neg[0 if (r[1] >> j) & 1 else 2, i * k + j] = r[2 + j]
+    pos, neg = decode_dbg(dbg.numpy()[:int(n_pos)], t1, t2, k)
     b = make()
     b.score_fed(_t(pos), _t(neg))
     assert a.read_loss() == pytest.approx(b.read_loss(), rel=1e-5)
@@ -297,17 +286,17 @@ def test_emulated_octet_scorer_replays_through_the_fed_scorer(cpu_engine_oct):
 
 
 @pytest.mark.parametrize("opt", ["Adagrad", "SGD"])
-def test_emulated_one_launch_step_equals_score_then_optimiser(cpu_engine_oct, monkeypatch, opt):
-    """k_step_sampled_oct (the bench's headline kernel: score + grid barrier + octet row optimiser in one cooperative
-    launch) against the two-launch path (octet scorer, then k_rowopt_pair) with the same sampling seed."""
+def test_emulated_one_launch_step_equals_score_then_optimiser(cpu_engine, octet_k, opt):
+    """k_step_sampled_duo / k_step_sampled_oct (score + grid barrier + flagged-row optimiser in one cooperative launch;
+    the duo is the bench's headline kernel) against the two-launch path (the same scorer, then k_rowopt_pair) with the
+    same sampling seed."""
     rng = np.random.default_rng(19)
-    t1, t2, kg1, kg2, tset, make = _sampled_setup(cpu_engine_oct, rng, opt)
+    t1, t2, kg1, kg2, tset, make = _sampled_setup(cpu_engine, rng, opt)
     fused, split = make(), make()
     for step in range(3):
-        fused.step_sampled(kg1, kg2, tset, 32, 6, step, 777)
-    monkeypatch.setenv("OEA_NO_FUSE", "1")
-    for step in range(3):
-        split.step_sampled(kg1, kg2, tset, 32, 6, step, 777)
+        fused.step_sampled(kg1, kg2, tset, 32, octet_k, step, 777)
+        split.score_sampled(kg1, kg2, tset, 32, octet_k, step, 777)
+        split.apply()
     assert fused.read_loss() == pytest.approx(split.read_loss(), rel=1e-5)
     for x, y in ((fused.ent, split.ent), (fused.rel, split.rel)):
         np.testing.assert_allclose(x.raw().numpy(), y.raw().numpy(), rtol=1e-4, atol=1e-6)

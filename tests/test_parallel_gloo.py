@@ -134,7 +134,6 @@ def _modes_worker(rank, world, port, out):
                     fn = getattr(lib, name); fn.restype, fn.argtypes = res, args
             L.load = lambda: lib
             eng._stream_ptr = lambda: C.c_void_p(0)
-            os.environ["OEA_NO_FUSE"] = "1"
             rng = np.random.default_rng(3)
             n, n_rel, d = 60, 5, 12
 

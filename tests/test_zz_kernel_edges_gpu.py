@@ -19,12 +19,6 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-@pytest.fixture(autouse=True)
-def _env(monkeypatch):
-    for var in ("OEA_NO_FUSE", "OEA_SCORE_V1", "OEA_SCORE_DUO"):
-        monkeypatch.delenv(var, raising=False)
-
-
 def _wave(dev):
     """Warps in one resident wave: 64 per SM."""
     return torch.cuda.get_device_properties(dev).multi_processor_count * 64
@@ -32,14 +26,13 @@ def _wave(dev):
 
 @pytest.mark.parametrize("loss_norm", ["L2", "L1"])
 @pytest.mark.parametrize("d", kc.DIMS)
-def test_fed_scorers_at_every_width(cuda_device, monkeypatch, d, loss_norm):
+def test_fed_scorers_at_every_width(cuda_device, d, loss_norm):
     for loss, k in kc.LOSSES:
         kc.check_fed(eng, cuda_device, d, loss_norm, loss, k, seed=d + k)
         kc.check_fed(eng, cuda_device, d, loss_norm, loss, k, seed=d + k, grouped=True)
-        if loss_norm == "L2" and d <= 128:
-            monkeypatch.setenv("OEA_SCORE_DUO", "0")
-            kc.check_fed(eng, cuda_device, d, loss_norm, loss, k, seed=d + k, grouped=True)
-            monkeypatch.delenv("OEA_SCORE_DUO")
+    if loss_norm == "L2" and d <= 128:                  # k_score_fed_grouped: k = 17 is past the duo
+        for loss in ("limited", "logistic"):
+            kc.check_fed(eng, cuda_device, d, loss_norm, loss, 17, seed=d + 17, grouped=True)
     scale = 6.0 if loss_norm == "L2" else 70.0 / np.sqrt(d)
     for loss, k in (("logistic", 2), ("logsigmoid", 0)):
         for grouped in (False, True):
@@ -85,14 +78,13 @@ def test_one_launch_fed_step_past_three_waves(cuda_device, opt):
                               n_ent=20000)
 
 
-def test_sampled_scorers_past_three_waves(cuda_device, monkeypatch):
+def test_sampled_scorers_past_three_waves(cuda_device):
     wave = _wave(cuda_device)
     big = dict(n_tri=14 * wave, n=20000, ref_dev=cuda_device)       # step 1 starts past the first batch
     m = kc.check_sampled(eng, cuda_device, 100, "L2", "limited", 10, 6 * wave + 200, seed=1, **big)      # duo
     assert (m + 1) // 2 > 3 * wave
     m = kc.check_sampled(eng, cuda_device, 100, "L2", "limited", 20, 3 * wave + 200, seed=2, **big)      # octet: k > 16
     assert m > 3 * wave
-    monkeypatch.setenv("OEA_SCORE_V1", "1")
     m = kc.check_sampled(eng, cuda_device, 300, "L1", "limited", 4, 3 * wave + 200, seed=3, **big)       # warp per positive
     assert m > 3 * wave
 
@@ -106,14 +98,11 @@ def test_one_launch_fed_step_equals_dense_steps(cuda_device, d, opt):
 
 @pytest.mark.parametrize("variant,d,loss_norm,loss,k", [
     ("duo", 1, "L2", "limited", 6), ("duo", 4, "L2", "margin-based", 1), ("duo", 127, "L2", "logistic", 3),
-    ("duo", 128, "L2", "limited", 16), ("oct", 3, "L2", "limited", 20), ("oct", 128, "L2", "logistic", 4),
+    ("duo", 128, "L2", "limited", 16), ("oct", 3, "L2", "limited", 20), ("oct", 128, "L2", "logistic", 17),
     ("v1", 129, "L1", "limited", 3), ("v1", 256, "L2", "logistic", 2), ("v1", 257, "L1", "margin-based", 1),
     ("v1", 384, "L2", "limited", 3), ("v1", 385, "L1", "logistic", 2), ("v1", 512, "L1", "limited", 3),
     ("v1", 512, "L2", "positive", 0)])
-def test_sampled_scorers_replay_through_the_reference(cuda_device, monkeypatch, variant, d, loss_norm, loss, k):
-    monkeypatch.setenv("OEA_SCORE_DUO", "0" if variant == "oct" else "1")
-    if variant == "v1":
-        monkeypatch.setenv("OEA_SCORE_V1", "1")
+def test_sampled_scorers_replay_through_the_reference(cuda_device, variant, d, loss_norm, loss, k):
     kc.check_sampled(eng, cuda_device, d, loss_norm, loss, k, 33, seed=d + k)
 
 
@@ -151,10 +140,10 @@ def test_optimisers_at_every_width(cuda_device, d, opt):
 
 
 # The one-launch sampled step of the duo kernel (k <= 16) and of the octet kernel (k > 16), in the order given, each
-# against the two-launch path (OEA_NO_FUSE=1) on the same batch.  A batch of 20 000 positives is more than three duo
+# against the two-launch path (the same scorer, then the row optimiser) on the same batch.  A batch of 20 000 positives is more than three duo
 # waves of pairs at 5 CTAs × 4 warps on 132 SMs (7 920 pairs).
 ORDER_SCRIPT = r"""
-import os, sys
+import sys
 import numpy as np, torch
 from openea_b200 import engine as eng
 from tests import kernel_edge_cases as kc
@@ -166,10 +155,9 @@ for kind in order:
     k = 10 if kind == "duo" else 20
     fused, split = make(), make()
     n_pos = torch.zeros(1, dtype=torch.int32, device="cuda")
-    os.environ["OEA_NO_FUSE"] = "0"
     fused.step_sampled(kg1, kg2, tset, 20000, k, 0, 99, n_pos_out=n_pos)
-    os.environ["OEA_NO_FUSE"] = "1"
-    split.step_sampled(kg1, kg2, tset, 20000, k, 0, 99)
+    split.score_sampled(kg1, kg2, tset, 20000, k, 0, 99)
+    split.apply()
     torch.cuda.synchronize()
     assert int(n_pos.item()) == 20000
     assert abs(fused.read_loss() - split.read_loss()) <= 1e-5 * abs(split.read_loss()), kind
@@ -187,8 +175,6 @@ print("ok")
 def test_one_launch_sampled_steps_in_either_order(cuda_device, order, opt):
     """The duo and octet one-launch steps have the same parameter list but different launch bounds (5 against 6 CTAs
     of 4 warps): whichever runs first in a process must not fix the cooperative grid of the other."""
-    env = dict(os.environ)
-    env.pop("OEA_NO_FUSE", None)
-    res = subprocess.run([sys.executable, "-c", ORDER_SCRIPT, order, opt], cwd=ROOT, env=env, capture_output=True,
-                         text=True, timeout=600)
+    res = subprocess.run([sys.executable, "-c", ORDER_SCRIPT, order, opt], cwd=ROOT, capture_output=True, text=True,
+                         timeout=600)
     assert res.returncode == 0 and res.stdout.strip().endswith("ok"), res.stdout[-2000:] + res.stderr[-4000:]

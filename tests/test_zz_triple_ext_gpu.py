@@ -217,11 +217,10 @@ def test_batch_producer_properties(cuda_device, sampler, k):
         assert dup_rows <= 0.01 * len(allp)
 
 
-def test_fast_batch_producer_draws_the_same_negatives_as_the_fused_kernel(cuda_device, monkeypatch):
+def test_fast_batch_producer_draws_the_same_negatives_as_the_fused_kernel(cuda_device):
     """sampler 0 shares warp_sample_negatives and the positive permutation with k_score_sampled: for one seed the
-    index vectors equal the fused kernel's debug dump."""
+    index vectors equal the fused kernel's debug dump (the L1 score: the warp-per-positive kernel)."""
     eng = _engine()
-    monkeypatch.setenv("OEA_SCORE_V1", "1")          # the warp-per-positive fused kernel
     rng = np.random.default_rng(23)
     t1, t2, n = _tiny_kgs(rng)
     ent = eng.EmbeddingTable(rng.standard_normal((2 * n, 16)).astype(np.float32), True)
@@ -229,7 +228,7 @@ def test_fast_batch_producer_draws_the_same_negatives_as_the_fused_kernel(cuda_d
     kg1 = eng.DeviceKG(t1, np.arange(0, n), 2 * n)
     kg2 = eng.DeviceKG(t2, np.arange(n, 2 * n), 2 * n)
     tset = eng.DeviceTripleSet([kg1.triples, kg2.triples], 2 * n, 11)
-    cfg = eng.loss_cfg("limited", "L2", 0.1, 2.0, 0.2)
+    cfg = eng.loss_cfg("limited", "L1", 0.1, 2.0, 0.2)
     B, k, step, seed = 256, 5, 2, 777
     dbg = torch.zeros(B, 2 + k, dtype=torch.int32, device="cuda")
     eng.TripleTrainer(ent, rel, cfg, 0.01).score_sampled(kg1, kg2, tset, B, k, step, seed, dbg=dbg)
