@@ -22,6 +22,15 @@
 #define OEA_LAUNCH(KERNEL, GRID, BLOCK, SMEM, STREAM, ...) KERNEL<<<(GRID), (BLOCK), (SMEM), (STREAM)>>>(__VA_ARGS__)
 #endif
 
+// OEA_LAUNCH of a grid-stride kernel (one that covers its work whatever the grid).  Under tests/emu it runs on at most
+// two blocks, which keeps the emulated thread count small.
+#ifdef OEA_HOST_EMU
+#define OEA_LAUNCH_STRIDED(KERNEL, GRID, BLOCK, SMEM, STREAM, ...) \
+    OEA_LAUNCH(KERNEL, ((GRID) < 2 ? (GRID) : 2), BLOCK, SMEM, STREAM, __VA_ARGS__)
+#else
+#define OEA_LAUNCH_STRIDED OEA_LAUNCH
+#endif
+
 // Cooperative launch (the kernel uses cooperative_groups::this_grid().sync()); the arguments must be lvalues of exactly
 // the kernel's parameter types.  Under tests/emu the grid is ONE block (every kernel launched this way walks its work
 // with grid-stride loops) and the grid barrier is that block's barrier.

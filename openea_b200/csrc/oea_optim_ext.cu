@@ -53,13 +53,8 @@ extern "C" int oea_rowopt_adadelta(const oea_table* t, const oea_opt_cfg* opt, v
     const int cap = sm_count_cached() * 8;
     const int grid = (int)(want < 1 ? 1 : (want < cap ? want : cap));
     const float rho = opt->beta1, eps = opt->eps;     // oea_opt_cfg: beta1 carries rho for Adadelta
-#ifdef OEA_HOST_EMU   // tests/emu: the same kernel on the CPU warp emulator
-    emu::launch(grid < 2 ? grid : 2, 256, [&] {
-        k_rowopt_adadelta(t->weight, t->grad, t->state1, t->state2, t->touched, t->rows, n4, opt->lr, rho, eps); });
-#else
-    k_rowopt_adadelta<<<grid, 256, 0, (cudaStream_t)stream>>>(t->weight, t->grad, t->state1, t->state2, t->touched,
-                                                               t->rows, n4, opt->lr, rho, eps);
-#endif
+    OEA_LAUNCH_STRIDED(k_rowopt_adadelta, grid, 256, 0, (cudaStream_t)stream, t->weight, t->grad, t->state1, t->state2,
+                       t->touched, t->rows, n4, opt->lr, rho, eps);
     OEA_LAUNCH_CHECK();
     return OEA_OK;
 }

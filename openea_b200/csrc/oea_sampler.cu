@@ -97,12 +97,8 @@ extern "C" int oea_triple_sample_batch(const oea_kg_view* kg1, const oea_kg_view
     P.diag = 0;
     const float* warm_w = warm ? warm->weight : nullptr;
     const int warm_pitch = warm ? warm->pitch : 0;
-#ifdef OEA_HOST_EMU   // tests/emu: the same kernel on the CPU warp emulator
-    emu::launch(grid_for(n_pos) < 2 ? grid_for(n_pos) : 2, kThreads,
-                [&] { k_sample_batch(P, sampler, warm_w, warm_pitch, pos_hrt, neg_hrt); });
-#else
-    k_sample_batch<<<grid_for(n_pos), kThreads, 0, (cudaStream_t)stream>>>(P, sampler, warm_w, warm_pitch, pos_hrt, neg_hrt);
-#endif
+    OEA_LAUNCH_STRIDED(k_sample_batch, grid_for(n_pos), kThreads, 0, (cudaStream_t)stream, P, sampler, warm_w, warm_pitch,
+                       pos_hrt, neg_hrt);
     OEA_LAUNCH_CHECK();
     return OEA_OK;
 }

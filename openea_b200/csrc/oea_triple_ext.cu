@@ -491,12 +491,6 @@ extern "C" int oea_model_score_fed(const oea_model* model,
     const bool margin = loss->loss_kind == OEA_LOSS_MARGIN;
     cudaStream_t st = (cudaStream_t)stream;
 
-#ifdef OEA_HOST_EMU   // tests/emu: the same kernels on the CPU warp emulator (two blocks keep the thread count small)
-#define OEA_RUN(KERNEL, ...) emu::launch(grid < 2 ? grid : 2, kThreads, [&] { KERNEL(__VA_ARGS__); })
-#else
-#define OEA_RUN(KERNEL, ...) KERNEL<<<grid, kThreads, 0, st>>>(__VA_ARGS__)
-#endif
-
     // RotatE: the independent losses only (its own log-sigmoid pair is OEA_LOSS_LOGISTIC); score_kind is not read
     if (model->kind == OEA_MODEL_ROTATE) {
         if (margin) return OEA_ERR_KIND;
@@ -504,10 +498,10 @@ extern "C" int oea_model_score_fed(const oea_model* model,
         const int grid = grid_for(n_pos + n_neg);
         if (model->ent->pitch <= 128) {
             auto kernel = k_model_fed<OEA_MODEL_ROTATE, OEA_SCORE_L2SQ, 1>;
-            OEA_RUN(kernel, M, pos_h, pos_r, pos_t, n_pos, neg_h, neg_r, neg_t, n_neg, *loss, loss_scale, loss_out);
+            OEA_LAUNCH_STRIDED(kernel, grid, kThreads, 0, st, M, pos_h, pos_r, pos_t, n_pos, neg_h, neg_r, neg_t, n_neg, *loss, loss_scale, loss_out);
         } else {
             auto kernel = k_model_fed<OEA_MODEL_ROTATE, OEA_SCORE_L2SQ, 2>;
-            OEA_RUN(kernel, M, pos_h, pos_r, pos_t, n_pos, neg_h, neg_r, neg_t, n_neg, *loss, loss_scale, loss_out);
+            OEA_LAUNCH_STRIDED(kernel, grid, kThreads, 0, st, M, pos_h, pos_r, pos_t, n_pos, neg_h, neg_r, neg_t, n_neg, *loss, loss_scale, loss_out);
         }
         OEA_LAUNCH_CHECK();
         return OEA_OK;
@@ -521,10 +515,10 @@ extern "C" int oea_model_score_fed(const oea_model* model,
         const int grid = grid_for(n_pos);
         if (model->ent->pitch <= 128) {
             auto kernel = k_hole_margin<1>;
-            OEA_RUN(kernel, M, pos_h, pos_r, pos_t, neg_h, neg_r, neg_t, n_pos, k, *loss, loss_scale, loss_out);
+            OEA_LAUNCH_STRIDED(kernel, grid, kThreads, 0, st, M, pos_h, pos_r, pos_t, neg_h, neg_r, neg_t, n_pos, k, *loss, loss_scale, loss_out);
         } else {
             auto kernel = k_hole_margin<2>;
-            OEA_RUN(kernel, M, pos_h, pos_r, pos_t, neg_h, neg_r, neg_t, n_pos, k, *loss, loss_scale, loss_out);
+            OEA_LAUNCH_STRIDED(kernel, grid, kThreads, 0, st, M, pos_h, pos_r, pos_t, neg_h, neg_r, neg_t, n_pos, k, *loss, loss_scale, loss_out);
         }
         OEA_LAUNCH_CHECK();
         return OEA_OK;
@@ -539,9 +533,9 @@ extern "C" int oea_model_score_fed(const oea_model* model,
 #define OEA_LAUNCH_MODEL(MODEL, SCORE, V)                                                                              \
     do {                                                                                                               \
         if (margin) { auto kernel = k_model_margin<MODEL, SCORE, V>;                                                   \
-                      OEA_RUN(kernel, M, pos_h, pos_r, pos_t, neg_h, neg_r, neg_t, n_pos, *loss, loss_scale, loss_out); } \
+                      OEA_LAUNCH_STRIDED(kernel, grid, kThreads, 0, st, M, pos_h, pos_r, pos_t, neg_h, neg_r, neg_t, n_pos, *loss, loss_scale, loss_out); } \
         else { auto kernel = k_model_fed<MODEL, SCORE, V>;                                                             \
-               OEA_RUN(kernel, M, pos_h, pos_r, pos_t, n_pos, neg_h, neg_r, neg_t, n_neg, *loss, loss_scale, loss_out); } \
+               OEA_LAUNCH_STRIDED(kernel, grid, kThreads, 0, st, M, pos_h, pos_r, pos_t, n_pos, neg_h, neg_r, neg_t, n_neg, *loss, loss_scale, loss_out); } \
     } while (0)
 #define OEA_LAUNCH_VEC(MODEL, SCORE)                                                  \
     do {                                                                              \
@@ -564,7 +558,6 @@ extern "C" int oea_model_score_fed(const oea_model* model,
 #undef OEA_LAUNCH_SCORE
 #undef OEA_LAUNCH_VEC
 #undef OEA_LAUNCH_MODEL
-#undef OEA_RUN
     OEA_LAUNCH_CHECK();
     return OEA_OK;
 }

@@ -425,18 +425,14 @@ extern "C" int oea_transr_score_fed(const oea_model* model,
     cudaStream_t st = (cudaStream_t)stream;
     const bool l1 = loss->score_kind == OEA_SCORE_L1;
 
-#ifdef OEA_HOST_EMU   // tests/emu: grid-stride kernels on two blocks keep the emulated thread count small
-    const int items_grid = 2, chunk_grid = 2;
-#else
     const int items_grid = grid_for((n + OEA_WARP - 1) / OEA_WARP);        // one thread per triple
     // ⌈n / C⌉ + min(R, n) chunks at most; the surplus CTAs see the device-side count and exit
     const int chunk_grid = (n + kTransrChunk - 1) / kTransrChunk + (n < rel->rows ? n : rel->rows);
-#endif
     OEA_CUDA_TRY(cudaMemsetAsync(hist, 0, sizeof(int32_t) * (size_t)rel->rows, st));
-    OEA_LAUNCH(k_transr_count, items_grid, kThreads, 0, st, B, hist, ticket);
+    OEA_LAUNCH_STRIDED(k_transr_count, items_grid, kThreads, 0, st, B, hist, ticket);
     OEA_LAUNCH(k_transr_plan, 1, kThreads, 0, st, hist, rel->rows, offs, chunks, n_chunks);
-    OEA_LAUNCH(k_transr_scatter, items_grid, kThreads, 0, st, B, offs, ticket, tmp);
-    OEA_LAUNCH(k_transr_stable, items_grid, kThreads, 0, st, B, hist, offs, tmp, order);
+    OEA_LAUNCH_STRIDED(k_transr_scatter, items_grid, kThreads, 0, st, B, offs, ticket, tmp);
+    OEA_LAUNCH_STRIDED(k_transr_stable, items_grid, kThreads, 0, st, B, hist, offs, tmp, order);
     OEA_LAUNCH_CHECK();
 
     const int smem_f = transr_smem_fwd(T.pitch), smem_b = transr_smem_bwd(T.pitch);
@@ -444,9 +440,9 @@ extern "C" int oea_transr_score_fed(const oea_model* model,
     auto bwd = l1 ? k_transr_bwd<OEA_SCORE_L1> : k_transr_bwd<OEA_SCORE_L2SQ>;
     OEA_CUDA_TRY(cudaFuncSetAttribute(fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_f));
     OEA_CUDA_TRY(cudaFuncSetAttribute(bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_b));
-    OEA_LAUNCH(fwd, chunk_grid, kThreads, smem_f, st, T, B, chunks, n_chunks, order, energy, proj);
-    OEA_LAUNCH(k_transr_loss, items_grid, kThreads, 0, st, energy, dloss, n_pos, n_neg, *loss, loss_scale, loss_out);
-    OEA_LAUNCH(bwd, chunk_grid, kThreads, smem_b, st, T, B, chunks, n_chunks, order, dloss, proj);
+    OEA_LAUNCH_STRIDED(fwd, chunk_grid, kThreads, smem_f, st, T, B, chunks, n_chunks, order, energy, proj);
+    OEA_LAUNCH_STRIDED(k_transr_loss, items_grid, kThreads, 0, st, energy, dloss, n_pos, n_neg, *loss, loss_scale, loss_out);
+    OEA_LAUNCH_STRIDED(bwd, chunk_grid, kThreads, smem_b, st, T, B, chunks, n_chunks, order, dloss, proj);
     OEA_LAUNCH_CHECK();
     return OEA_OK;
 }

@@ -1,5 +1,5 @@
 // cuda_host_emu.h — TEST INFRASTRUCTURE: a warp-level CUDA execution model on the CPU, so that the product's kernel
-// sources (openea_b200/csrc/*.cu, compiled unchanged with -DOEA_HOST_EMU by g++) can be checked against the oracle
+// sources (openea_b200/csrc/*.cu, compiled unchanged by g++ with OEA_HOST_EMU defined) can be checked against the oracle
 // where no GPU exists.  Not a fallback: nothing under openea_b200/ ever loads a library built with it.
 //
 // Model: one OS thread per CUDA thread (a worker pool reused from block to block).  All warps of a block run concurrently; the 32 lanes of a warp meet at every
@@ -11,6 +11,7 @@
 // "Device" pointers are host pointers; atomics and red adds are real atomics (std::atomic_ref).
 #pragma once
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <math.h>
 #include <stdint.h>
 #include <string.h>
@@ -260,6 +261,8 @@ inline void __syncwarp(unsigned mask = 0xffffffffu) { emu::sync(mask); }     // 
 template <typename T>
 inline T __ldg(const T* p) { return *p; }
 template <typename T>
+inline T __ldcg(const T* p) { return std::atomic_ref<T>(*const_cast<T*>(p)).load(std::memory_order_relaxed); }
+template <typename T>
 inline T emu_atomic_rmw(T* p, T (*op)(T, T), T v) {
     std::atomic_ref<T> a(*p);
     T old = a.load(std::memory_order_relaxed);
@@ -275,6 +278,7 @@ inline unsigned long long atomicMax(unsigned long long* p, unsigned long long v)
 }
 inline unsigned atomicMax(unsigned* p, unsigned v) { return emu_atomic_rmw<unsigned>(p, [](unsigned a, unsigned b) { return a > b ? a : b; }, v); }
 inline int atomicMax(int* p, int v) { return emu_atomic_rmw<int>(p, [](int a, int b) { return a > b ? a : b; }, v); }
+inline int atomicMin(int* p, int v) { return emu_atomic_rmw<int>(p, [](int a, int b) { return a < b ? a : b; }, v); }
 inline float atomicAdd(float* p, float v) {          // lanes of one warp may hit the same word (scatter-adds): really atomic
     std::atomic_ref<float> a(*p);
     float old = a.load(std::memory_order_relaxed);

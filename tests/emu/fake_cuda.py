@@ -9,7 +9,6 @@ this way are meaningless as measurements.  Only tests/test_bench_on_emulator.py 
     python tests/emu/fake_cuda.py lifecycle <Approach> <tmp folder>
     python tests/emu/fake_cuda.py pytest <pytest arguments…>      (ad-hoc: GPU-marked tests against the emulator)
 """
-import ctypes as C
 import os
 import sys
 import time
@@ -17,23 +16,16 @@ import types
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
+import pytest  # noqa: E402
 import torch  # noqa: E402
 
 from openea_b200 import engine as eng  # noqa: E402
 from openea_b200 import finding  # noqa: E402
-from openea_b200 import lib as L  # noqa: E402
 from tests.emu import build_emu  # noqa: E402
 
 
 def install():
-    lib = C.CDLL(build_emu.build())
-    for name, (res, args) in L.SIGNATURES.items():
-        if hasattr(lib, name):
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = res, args
-    L.load = lambda: lib
-    null = lambda: C.c_void_p(0)
-    eng._stream_ptr = finding._stream_ptr = null
+    build_emu.patch_engine(pytest.MonkeyPatch(), build_emu.load())      # for the life of the process
     cpu = torch.device("cpu")
 
     class Stream:
@@ -174,7 +166,6 @@ def main():
     if what == "lifecycle":
         return lifecycle(rest[0], rest[1])
     if what == "pytest":                     # ad-hoc audits: GPU-marked tests executed against the emulator
-        import pytest
         return pytest.main(rest)
     if what == "smoke":
         import __graft_entry__

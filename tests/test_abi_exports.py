@@ -1,6 +1,11 @@
-"""CPU: the C-ABI library is built, loads without a GPU, and exports every symbol include/oea.h declares."""
+"""CPU: the C-ABI library is built, loads without a GPU, and exports every symbol include/oea.h declares; so does the
+emulated library of tests/emu."""
 import ctypes
+import glob
 import os
+import re
+
+import pytest
 
 from openea_b200 import lib as L
 
@@ -13,6 +18,22 @@ def test_header_symbols_all_bound_and_exported():
     raw = ctypes.CDLL(L.LIB_PATH)
     for name in declared:
         assert hasattr(raw, name), "liboea.so does not export " + name
+
+
+def test_emulated_library_includes_every_kernel_source_and_exports_every_symbol():
+    """tests/emu/emu_kernels.cpp includes every openea_b200/csrc/*.cu, so no entry point is out of the emulator's
+    reach, and the library built from it exports every symbol include/oea.h declares."""
+    from tests.emu import build_emu
+    with open(build_emu.SRC) as f:
+        included = set(re.findall(r'^#include "\.\./\.\./openea_b200/csrc/(\w+\.cu)"', f.read(), flags=re.M))
+    sources = {os.path.basename(p) for p in glob.glob(os.path.join(build_emu.CSRC, "*.cu"))}
+    assert included == sources, "emu_kernels.cpp misses %s" % sorted(sources - included)
+    path = build_emu.build()
+    if path is None:
+        pytest.skip("no CUDA headers for the emulator build")
+    raw = ctypes.CDLL(path)
+    missing = [name for name in L.declared_symbols() if not hasattr(raw, name)]
+    assert not missing, "the emulated library does not export " + ", ".join(missing)
 
 
 def test_load_and_error_strings_without_gpu():

@@ -1,7 +1,7 @@
 """CPU: the Python host layer of the score-function family (openea_b200.engine.ModelTrainer, DeviceKG,
 DeviceTripleSet — ctypes structs, pointer lifetimes, buffer slicing, step sequencing) driven end to end over CPU
-tensors, with the two emulated entry points served by the warp emulator (tests/emu) and the entry points whose
-kernels are not emulated (row optimiser, triple-set build) served by NumPy statements of their documented contract.
+tensors, with two entry points served by the warp emulator (tests/emu) and two (row optimiser, triple-set build) by
+NumPy statements of their documented contract.
 Only this test wires the engine this way; the product path loads liboea.so and nothing else."""
 import ctypes as C
 
@@ -27,9 +27,7 @@ class HybridLib:
 
     def __init__(self, emu):
         for name in ("oea_model_score_fed", "oea_triple_sample_batch"):
-            fn = getattr(emu, name)
-            fn.restype, fn.argtypes = L.SIGNATURES[name]
-            setattr(self, name, fn)
+            setattr(self, name, getattr(emu, name))
 
     @staticmethod
     def oea_error_string(rc):
@@ -64,12 +62,7 @@ class HybridLib:
 
 @pytest.fixture()
 def cpu_engine(monkeypatch):
-    so = build_emu.build()
-    if so is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    hybrid = HybridLib(C.CDLL(so))
-    monkeypatch.setattr(L, "load", lambda: hybrid)
-    monkeypatch.setattr(eng, "_stream_ptr", lambda: C.c_void_p(0))
+    build_emu.patch_engine(monkeypatch, HybridLib(build_emu.load()))
     return eng
 
 

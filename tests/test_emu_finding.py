@@ -3,14 +3,12 @@ CSLS on the stored matrix, row / column top-k means, radix selection of the k ne
 their SOURCE on the warp emulator (all warps of a block concurrent, real __syncthreads) through the
 product's own host layer (openea_b200/finding.py over CPU tensors), against the golden vectors the reference itself
 produced (tests/golden/finding_golden.npz).  The same checks run on the GPU in tests/test_finding_gpu.py."""
-import ctypes as C
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from openea_b200 import lib as L
 from tests.emu import build_emu
 
 GOLD = np.load(os.path.join(os.path.dirname(__file__), "golden", "finding_golden.npz"))
@@ -18,20 +16,9 @@ GOLD = np.load(os.path.join(os.path.dirname(__file__), "golden", "finding_golden
 
 @pytest.fixture()
 def finding_cpu(monkeypatch):
-    so = build_emu.build()
-    if so is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    lib = C.CDLL(so)
-    for name, (res, args) in L.SIGNATURES.items():
-        if hasattr(lib, name):
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = res, args
-    from openea_b200 import engine as eng
     from openea_b200 import finding
-    monkeypatch.setattr(L, "load", lambda: lib)
+    build_emu.patch_engine(monkeypatch, build_emu.load())
     monkeypatch.setattr(finding, "_device", lambda: torch.device("cpu"))
-    monkeypatch.setattr(finding, "_stream_ptr", lambda: C.c_void_p(0))
-    monkeypatch.setattr(eng, "_stream_ptr", lambda: C.c_void_p(0))
     return finding
 
 

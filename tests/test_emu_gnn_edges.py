@@ -10,26 +10,14 @@ import ctypes as C
 import pytest
 import torch
 
-from openea_b200 import lib as L
 from tests import gnn_edge_cases as gc
 from tests.emu import build_emu
 
 
 @pytest.fixture()
 def dev(monkeypatch):
-    so = build_emu.build()
-    if so is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    lib = C.CDLL(so)
-    for name, (res, args) in L.SIGNATURES.items():
-        if hasattr(lib, name):
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = res, args
-    from openea_b200 import engine as eng
-    from openea_b200 import gnn
-    monkeypatch.setattr(L, "load", lambda: lib)
-    monkeypatch.setattr(gnn, "_stream_ptr", lambda: C.c_void_p(0))
-    monkeypatch.setattr(eng, "_stream_ptr", lambda: C.c_void_p(0))
+    lib = build_emu.load()
+    build_emu.patch_engine(monkeypatch, lib)
     d = C.c_int(0)
     assert lib.cudaGetDevice(C.byref(d)) != 0, "a CUDA device is visible: the grid would not be sized by the fallback"
     return torch.device("cpu")

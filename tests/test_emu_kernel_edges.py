@@ -17,16 +17,8 @@ from tests.emu import build_emu
 
 @pytest.fixture()
 def cpu_engine(monkeypatch):
-    so = build_emu.build()
-    if so is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    lib = C.CDLL(so)
-    for name, (res, args) in L.SIGNATURES.items():
-        if hasattr(lib, name):
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = res, args
-    monkeypatch.setattr(L, "load", lambda: lib)
-    monkeypatch.setattr(eng, "_stream_ptr", lambda: C.c_void_p(0))
+    lib = build_emu.load()
+    build_emu.patch_engine(monkeypatch, lib)
     return eng, lib
 
 

@@ -5,20 +5,12 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from openea_b200 import lib as L
 from tests.emu import build_emu
 
 
 @pytest.fixture(scope="module")
 def emu():
-    so = build_emu.build()
-    if so is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    lib = C.CDLL(so)
-    for name in ("oea_gale_shapley_workspace_bytes", "oea_gale_shapley", "oea_rows_gather_sort"):
-        fn = getattr(lib, name)
-        fn.restype, fn.argtypes = L.SIGNATURES[name]
-    return lib
+    return build_emu.load()
 
 
 def _host_matching(s, cut):

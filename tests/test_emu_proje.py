@@ -1,4 +1,4 @@
-"""CPU: ProjE's kernels (openea_b200/csrc/oea_proje.cu) on the warp emulator of tests/emu (tests/emu/build_emu_proje.py):
+"""CPU: ProjE's kernels (openea_b200/csrc/oea_proje.cu) on the warp emulator of tests/emu:
 the unique log-uniform sampler against the sequential loop over the same draw stream, the step's forward and backward
 against the float64 oracle of tests/proje_oracle.py (row widths, batch sizes down to one positive, sampled sets up to
 every class, repeated labels, labels inside the sampled set, TF's expected-count shortcut), whole Adam steps on the five
@@ -12,22 +12,12 @@ from scipy import stats
 
 from openea_b200 import lib as L
 from tests import proje_oracle as po
-from tests.emu import build_emu_proje
-
-
-def _bind(lib):
-    for name in ("oea_logu_sample_unique", "oea_proje_workspace_bytes", "oea_proje_score_fed", "oea_rowopt_apply"):
-        res, args = L.SIGNATURES[name]
-        getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
-    return lib
+from tests.emu import build_emu
 
 
 @pytest.fixture(scope="module")
 def emu():
-    so_path = build_emu_proje.build()
-    if so_path is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    return _bind(C.CDLL(so_path))
+    return build_emu.load()
 
 
 def _aligned(nbytes):

@@ -5,7 +5,6 @@ before the call.  The cooperative launch runs as one block here, so each warp wa
 Flagged rows must equal a NumPy float32 restatement of TF1 Adagrad / SGD; unflagged rows keep their weight, slot and
 gradient bit for bit; afterwards every flag and every flagged gradient row is zero and padding columns are unchanged
 (tests/rowopt_flag_cases.py has the patterns)."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -19,18 +18,8 @@ BASE_A, BASE_B = 1200, 17         # one block of 4 (duo) or 8 (grouped) warps: 7
 @pytest.fixture()
 def emu_engine(monkeypatch):
     from openea_b200 import engine as eng
-    from openea_b200 import lib as L
     from tests.emu import build_emu
-    so = build_emu.build()
-    if so is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    lib = C.CDLL(so)
-    for name, (res, args) in L.SIGNATURES.items():
-        if hasattr(lib, name):
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = res, args
-    monkeypatch.setattr(L, "load", lambda: lib)
-    monkeypatch.setattr(eng, "_stream_ptr", lambda: C.c_void_p(0))
+    build_emu.patch_engine(monkeypatch, build_emu.load())
     return eng
 
 

@@ -34,13 +34,7 @@ def build_tripleset(triples, ent_bits, rel_bits, capacity=None):
 
 @pytest.fixture(scope="module")
 def emu():
-    so = build_emu.build()
-    if so is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    lib = C.CDLL(so)
-    res, args = L.SIGNATURES["oea_triple_sample_batch"]
-    lib.oea_triple_sample_batch.restype, lib.oea_triple_sample_batch.argtypes = res, args
-    return lib
+    return build_emu.load()
 
 
 def _kgs(rng, n=60, n_rel=5, n_tri=260):

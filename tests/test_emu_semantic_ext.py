@@ -6,7 +6,6 @@ import ctypes as C
 import math
 import os
 import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -22,18 +21,9 @@ KINDS = {"RotatE": L.MODEL_ROTATE, "HolE": L.MODEL_HOLE}
 GAMMA = 12.0
 
 
-def _bind(lib):
-    res, args = L.SIGNATURES["oea_model_score_fed"]
-    lib.oea_model_score_fed.restype, lib.oea_model_score_fed.argtypes = res, args
-    return lib
-
-
 @pytest.fixture(scope="module")
 def emu():
-    so_path = build_emu.build()
-    if so_path is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    return _bind(C.CDLL(so_path))
+    return build_emu.load()
 
 
 def _case(model, seed, n_ent, n_rel, d, norm):
@@ -188,26 +178,17 @@ MUTATION = ("const float dth = fmaf(da, -fmaf(hr, sn, hi * cs), db * fmaf(hr, cs
 def test_emulated_rotate_phase_backward_mutation_is_caught(tmp_path):
     """The comparison with the oracle has teeth: the kernel source with one sign flipped in the phase backward
     (dθ's first term), built for the emulator, must disagree with the oracle on the relation gradient."""
-    inc = build_emu.cuda_include()
-    if inc is None:
+    if build_emu.cuda_include() is None:
         pytest.skip("no CUDA headers for the emulator build")
     csrc = tmp_path / "openea_b200" / "csrc"
     shutil.copytree(os.path.join(ROOT, "openea_b200", "csrc"), csrc)
     shutil.copytree(os.path.join(ROOT, "include"), tmp_path / "include")
-    (tmp_path / "tests" / "emu").mkdir(parents=True)
-    shutil.copy(os.path.join(ROOT, "tests", "emu", "cuda_host_emu.h"), tmp_path / "tests" / "emu")
     src = (csrc / "oea_triple_ext.cu").read_text()
     assert src.count(MUTATION[0]) == 1, "the mutated statement is not in the kernel source any more"
     (csrc / "oea_triple_ext.cu").write_text(src.replace(MUTATION[0], MUTATION[1]))
-    main = tmp_path / "tests" / "emu" / "mutant.cpp"
-    main.write_text('#include "cuda_host_emu.h"\n#include "../../openea_b200/csrc/oea_triple_ext.cu"\n')
-    out = tmp_path / "libmutant.so"
-    cmd = ["g++", "-std=c++20", "-O1", "-pthread", "-fPIC", "-shared", "-DOEA_HOST_EMU", "-Wno-attributes",
-           "-Wno-unknown-pragmas", "-I", inc, "-o", str(out), str(main),
-           "-L", os.path.join(os.path.dirname(inc), "lib64"), "-lcudart"]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[-3000:]
-    mutant = _bind(C.CDLL(str(out)))
+    main = tmp_path / "mutant.cpp"
+    main.write_text('#include "cuda_host_emu.h"\n#include "openea_b200/csrc/oea_triple_ext.cu"\n')
+    mutant = build_emu.load(build_emu.compile(str(main), str(tmp_path / "libmutant.so")), ["oea_model_score_fed"])
     d = 20
     rng, tabs, norms = _case("RotatE", 12, 30, 5, d, True)
     pos, neg = make_batch(rng, 30, 5, 13, 3)

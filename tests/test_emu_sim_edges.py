@@ -9,7 +9,6 @@ import numpy as np
 import pytest
 import torch
 
-from openea_b200 import lib as L
 from oracle import finding as orf
 from tests import sim_edge_cases as sc
 from tests.emu import build_emu
@@ -19,20 +18,10 @@ SHAPES = [(1, 127), (127, 128), (128, 129), (129, 255), (255, 257), (257, 1)]
 
 @pytest.fixture()
 def F(monkeypatch):
-    so = build_emu.build()
-    if so is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    lib = C.CDLL(so)
-    for name, (res, args) in L.SIGNATURES.items():
-        if hasattr(lib, name):
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = res, args
-    from openea_b200 import engine as eng
     from openea_b200 import finding
-    monkeypatch.setattr(L, "load", lambda: lib)
+    lib = build_emu.load()
+    build_emu.patch_engine(monkeypatch, lib)
     monkeypatch.setattr(finding, "_device", lambda: torch.device("cpu"))
-    monkeypatch.setattr(finding, "_stream_ptr", lambda: C.c_void_p(0))
-    monkeypatch.setattr(eng, "_stream_ptr", lambda: C.c_void_p(0))
     monkeypatch.delenv("OEA_SIM_TC", raising=False)
     monkeypatch.delenv("OEA_SIM_NO_SHORTK", raising=False)
     dev = C.c_int(0)

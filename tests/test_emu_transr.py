@@ -1,19 +1,18 @@
 """CPU: TransR's relation-grouped kernels (openea_b200/csrc/oea_triple_transr.cu) executed on the warp emulator of
-tests/emu (tests/emu/build_emu_transr.py) against the float64 oracle of tests/transr_oracle.py: every row width bucket, every loss and score, relations
+tests/emu against the float64 oracle of tests/transr_oracle.py: every row width bucket, every loss and score, relations
 split over several chunks, relations absent from the batch, negatives with another relation than their positive,
 degenerate rows, the argument checks, the initialisation's scale, and a source mutation the comparison must catch."""
 import ctypes as C
 import math
 import os
 import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 from openea_b200 import lib as L
 from tests import transr_oracle as tro
-from tests.emu import build_emu, build_emu_transr
+from tests.emu import build_emu
 from tests.helpers import make_batch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -22,19 +21,9 @@ LOSSES = {"margin-based": L.LOSS_MARGIN, "limited": L.LOSS_LIMITED, "logistic": 
           "positive": L.LOSS_POSITIVE}
 
 
-def _bind(lib):
-    for name in ("oea_transr_score_fed", "oea_transr_workspace_bytes", "oea_model_score_fed", "oea_rowopt_apply"):
-        res, args = L.SIGNATURES[name]
-        getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
-    return lib
-
-
 @pytest.fixture(scope="module")
 def emu():
-    so_path = build_emu_transr.build()
-    if so_path is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    return _bind(C.CDLL(so_path))
+    return build_emu.load()
 
 
 class HostTable:
@@ -258,29 +247,18 @@ MUTATION = ("tile_gemm(acc, Gs, ld, 1, Ms, ld, 1, d, ty, tx);          // dX[j][
 def test_emulated_transr_transposed_backward_mutation_is_caught(tmp_path):
     """The comparison with the oracle has teeth: the kernel source with M_r instead of M_rᵀ in dĥ / dt̂, built for the
     emulator, must disagree with the oracle on the entity gradient, while the matrix gradient still agrees."""
-    inc = build_emu.cuda_include()
-    if inc is None:
+    if build_emu.cuda_include() is None:
         pytest.skip("no CUDA headers for the emulator build")
     csrc = tmp_path / "openea_b200" / "csrc"
     shutil.copytree(os.path.join(ROOT, "openea_b200", "csrc"), csrc)
     shutil.copytree(os.path.join(ROOT, "include"), tmp_path / "include")
-    (tmp_path / "tests" / "emu").mkdir(parents=True)
-    shutil.copy(os.path.join(ROOT, "tests", "emu", "cuda_host_emu.h"), tmp_path / "tests" / "emu")
     src = (csrc / "oea_triple_transr.cu").read_text()
     assert src.count(MUTATION[0]) == 1, "the mutated statement is not in the kernel source any more"
     (csrc / "oea_triple_transr.cu").write_text(src.replace(MUTATION[0], MUTATION[1]))
-    main = tmp_path / "tests" / "emu" / "mutant.cpp"
-    main.write_text('#include "cuda_host_emu.h"\n#include "../../openea_b200/csrc/oea_triple_transr.cu"\n')
-    out = tmp_path / "libmutant.so"
-    cmd = ["g++", "-std=c++20", "-O1", "-pthread", "-fPIC", "-shared", "-DOEA_HOST_EMU", "-Wno-attributes",
-           "-Wno-unknown-pragmas", "-I", inc, "-o", str(out), str(main),
-           "-L", os.path.join(os.path.dirname(inc), "lib64"), "-lcudart"]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[-3000:]
-    mutant = C.CDLL(str(out))
-    for name in ("oea_transr_score_fed", "oea_transr_workspace_bytes"):
-        res_t, args = L.SIGNATURES[name]
-        getattr(mutant, name).restype, getattr(mutant, name).argtypes = res_t, args
+    main = tmp_path / "mutant.cpp"
+    main.write_text('#include "cuda_host_emu.h"\n#include "openea_b200/csrc/oea_triple_transr.cu"\n')
+    mutant = build_emu.load(build_emu.compile(str(main), str(tmp_path / "libmutant.so")),
+                            ["oea_transr_score_fed", "oea_transr_workspace_bytes"])
     d = 12
     rng, tabs, norms = _case(12, 30, 4, d)
     pos, neg = make_batch(rng, 30, 4, 13, 1)

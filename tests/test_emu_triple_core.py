@@ -19,16 +19,7 @@ from tests.kernel_edge_cases import decode_dbg
 
 @pytest.fixture()
 def cpu_engine(monkeypatch):
-    so = build_emu.build()
-    if so is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    lib = C.CDLL(so)
-    for name, (res, args) in L.SIGNATURES.items():
-        if hasattr(lib, name):
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = res, args
-    monkeypatch.setattr(L, "load", lambda: lib)
-    monkeypatch.setattr(eng, "_stream_ptr", lambda: C.c_void_p(0))
+    build_emu.patch_engine(monkeypatch, build_emu.load())
     return eng
 
 

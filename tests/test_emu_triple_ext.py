@@ -20,13 +20,7 @@ KINDS = {"TransE": L.MODEL_TRANSE, "TransH": L.MODEL_TRANSH, "TransD": L.MODEL_T
 
 @pytest.fixture(scope="module")
 def emu():
-    so = build_emu.build()
-    if so is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    lib = C.CDLL(so)
-    res, args = L.SIGNATURES["oea_model_score_fed"]
-    lib.oea_model_score_fed.restype, lib.oea_model_score_fed.argtypes = res, args
-    return lib
+    return build_emu.load()
 
 
 class HostTable:
@@ -121,8 +115,6 @@ def test_emulated_adadelta_update_matches_tf_rule(emu):
     """oea_rowopt_adadelta (openea_b200/csrc/oea_optim_ext.cu) on the emulator: three dense steps equal TF1's ApplyAdadelta
     (rho 0.95, epsilon 1e-8) on every row — rows without gradient decay their accumulators too — and leave grad /
     touched zeroed."""
-    res, args = L.SIGNATURES["oea_rowopt_adadelta"]
-    emu.oea_rowopt_adadelta.restype, emu.oea_rowopt_adadelta.argtypes = res, args
     rng = np.random.default_rng(2)
     rows, d = 37, 10                                            # pitch 12
     tab = HostTable(rng.standard_normal((rows, d)).astype(np.float32), False)

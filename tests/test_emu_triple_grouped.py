@@ -18,13 +18,7 @@ LOSSES = {"margin-based": L.LOSS_MARGIN, "limited": L.LOSS_LIMITED, "logistic": 
 
 @pytest.fixture(scope="module")
 def emu():
-    so = build_emu.build()
-    if so is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    lib = C.CDLL(so)
-    lib.oea_triple_score_fed_grouped.restype, lib.oea_triple_score_fed_grouped.argtypes = \
-        L.SIGNATURES["oea_triple_score_fed_grouped"]
-    return lib
+    return build_emu.load()
 
 
 def _run(emu, ent, rel, pos, neg, loss, loss_norm, **kw):

@@ -5,6 +5,7 @@ import os
 import socket
 
 import numpy as np
+import pytest
 import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
@@ -93,8 +94,7 @@ def _modes_worker(rank, world, port, out):
     os.environ["MASTER_PORT"] = str(port)
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
-        import ctypes as C
-        from openea_b200 import engine as eng, lib as L, parallel as par
+        from openea_b200 import engine as eng, parallel as par
         # ---- push() publishes, pull() applies: what happens to the table between the two does not leak into the peers' copies
         w = torch.full((41, 4), float(rank + 1))
         x = par.SeedRowSync(w, np.arange(0, 41, 3), rank, world)
@@ -128,12 +128,7 @@ def _modes_worker(rank, world, port, out):
         from tests.emu import build_emu
         so = build_emu.build()
         if so is not None:
-            lib = C.CDLL(so)
-            for name, (res, args) in L.SIGNATURES.items():
-                if hasattr(lib, name):
-                    fn = getattr(lib, name); fn.restype, fn.argtypes = res, args
-            L.load = lambda: lib
-            eng._stream_ptr = lambda: C.c_void_p(0)
+            build_emu.patch_engine(pytest.MonkeyPatch(), build_emu.load(so))
             rng = np.random.default_rng(3)
             n, n_rel, d = 60, 5, 12
 

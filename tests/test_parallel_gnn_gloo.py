@@ -81,15 +81,10 @@ class EmuOps(TorchOps):
 
     def __init__(self):
         import ctypes as C
-        from openea_b200 import lib as L
         from tests.emu import build_emu
         from tests.test_emu_spmm import HostCsr
-        self.C, self.L, self.HostCsr = C, L, HostCsr
-        self.lib = C.CDLL(build_emu.build())
-        for name in ("oea_spmm_csr", "oea_spmm_workspace_bytes", "oea_spmm_long_row_threshold", "oea_spmm_segment_nnz",
-                     "oea_align_loss_l1"):
-            fn = getattr(self.lib, name)
-            fn.restype, fn.argtypes = L.SIGNATURES[name]
+        self.C, self.HostCsr = C, HostCsr
+        self.lib = build_emu.load()
 
     def csr(self, mat, device, keep_duplicates=False):
         ops = self

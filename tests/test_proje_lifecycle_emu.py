@@ -1,7 +1,6 @@
 """CPU: ProjE's configuration and initialisation, and set_args / set_kgs / init / run / save on the micro synthetic
-dataset with the engine's entry points on the warp-emulator library of tests/emu/build_emu_proje.py (in-process, as
+dataset with the engine's entry points on the warp-emulator library of tests/emu (in-process, as
 tests/test_jape.py runs JAPE)."""
-import ctypes as C
 import math
 import os
 import re
@@ -11,9 +10,8 @@ import pytest
 import torch
 
 from openea_b200 import engine as eng
-from openea_b200 import lib as L
 from openea_b200 import presets
-from tests.emu import build_emu_proje
+from tests.emu import build_emu
 
 SHIPPED = {  # run/args/proje_args_15K.json and proje_args_100K.json, the keys the engine reads
     "15K": dict(embedding_module="ProjE", alignment_module="sharing", dim=100, init="xavier", ent_l2_norm=True,
@@ -48,16 +46,7 @@ def test_xavier_on_a_one_dimensional_shape():
 
 @pytest.fixture()
 def proje_engine(monkeypatch):
-    so = build_emu_proje.build()
-    if so is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    lib = C.CDLL(so)
-    for name, (res, args) in L.SIGNATURES.items():
-        if hasattr(lib, name):
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = res, args
-    monkeypatch.setattr(L, "load", lambda: lib)
-    monkeypatch.setattr(eng, "_stream_ptr", lambda: C.c_void_p(0))
+    build_emu.patch_engine(monkeypatch, build_emu.load())
     return eng
 
 

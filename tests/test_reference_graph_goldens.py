@@ -198,10 +198,7 @@ def replay_gcn_align(engine, device, branch):
 
 
 @pytest.mark.parametrize("branch", ["se", "ae"])
-def test_gcn_align_unit_on_the_emulator_reproduces_the_reference_unit(cpu_engine, monkeypatch, branch):
-    import ctypes as C
-    from openea_b200 import gnn
-    monkeypatch.setattr(gnn, "_stream_ptr", lambda: C.c_void_p(0))
+def test_gcn_align_unit_on_the_emulator_reproduces_the_reference_unit(cpu_engine, branch):
     replay_gcn_align(cpu_engine, "cpu", branch)
 
 
@@ -274,10 +271,7 @@ def replay_rdgcn(device):
         np.testing.assert_allclose(layer.forward()[:, :dim].cpu().numpy(), RD["outputs_final"], rtol=2e-3, atol=2e-5)
 
 
-def test_rdgcn_layer_on_the_emulator_reproduces_the_reference_layer(cpu_engine, monkeypatch):
-    import ctypes as C
-    from openea_b200 import gnn
-    monkeypatch.setattr(gnn, "_stream_ptr", lambda: C.c_void_p(0))
+def test_rdgcn_layer_on_the_emulator_reproduces_the_reference_layer(cpu_engine):
     replay_rdgcn("cpu")
 
 
@@ -333,10 +327,7 @@ def replay_alinet(device):
             np.testing.assert_allclose(out[:, :dims[i + 1]].cpu().numpy(), AL["outputs_final/%d" % i], rtol=2e-3, atol=2e-5)
 
 
-def test_alinet_model_on_the_emulator_reproduces_the_reference_graph(cpu_engine, monkeypatch):
-    import ctypes as C
-    from openea_b200 import gnn
-    monkeypatch.setattr(gnn, "_stream_ptr", lambda: C.c_void_p(0))
+def test_alinet_model_on_the_emulator_reproduces_the_reference_graph(cpu_engine):
     replay_alinet("cpu")
 
 

@@ -11,7 +11,6 @@ must reproduce every fetched loss within 2·10⁻⁴ and the variables after the
 
 tests/transr_oracle.py is pinned to the same file at float64 precision.
 """
-import ctypes as C
 import json
 import os
 import types
@@ -21,9 +20,8 @@ import pytest
 import torch
 
 from openea_b200 import engine as eng
-from openea_b200 import lib as L
 from tests import transr_oracle as tro
-from tests.emu import build_emu_transr
+from tests.emu import build_emu
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "path_i_transr.npz")
 G = np.load(GOLDEN)
@@ -82,17 +80,7 @@ def replay(case, engine, device, monkeypatch):
 
 @pytest.fixture()
 def cpu_engine(monkeypatch):
-    """The engine over the emulated library that includes the TransR kernels (tests/emu/build_emu_transr.py)."""
-    so = build_emu_transr.build()
-    if so is None:
-        pytest.skip("no CUDA headers for the emulator build")
-    lib = C.CDLL(so)
-    for name, (res, args) in L.SIGNATURES.items():
-        if hasattr(lib, name):
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = res, args
-    monkeypatch.setattr(L, "load", lambda: lib)
-    monkeypatch.setattr(eng, "_stream_ptr", lambda: C.c_void_p(0))
+    build_emu.patch_engine(monkeypatch, build_emu.load())
     return eng
 
 

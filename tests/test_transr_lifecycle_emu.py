@@ -1,6 +1,5 @@
 """CPU: set_args / set_kgs / init / run / test / save of TransR on the micro synthetic dataset, through
-tests/emu/fake_cuda.py (torch's CUDA surface faked, liboea's entry points on the warp emulator library of
-tests/emu/build_emu_transr.py), with presets.transr —
+tests/emu/fake_cuda.py (torch's CUDA surface faked, liboea's entry points on the warp emulator), with presets.transr —
 the values of the reference's run/args/transr_args_15K.json."""
 import os
 import subprocess
@@ -9,7 +8,7 @@ import sys
 import pytest
 
 from openea_b200 import presets
-from tests.emu import build_emu_transr
+from tests.emu import build_emu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 RUNNER = os.path.join(ROOT, "tests", "emu", "fake_cuda.py")
@@ -23,12 +22,10 @@ def test_transr_preset_is_the_shipped_configuration():
 
 
 def test_transr_lifecycle_on_the_emulator(tmp_path):
-    lib = build_emu_transr.build()
-    if lib is None:
+    if build_emu.build() is None:
         pytest.skip("no CUDA headers for the emulator build")
-    env = dict(os.environ, OEA_EMU_LIB=lib)           # the runner's emulated library, with the TransR entry points
     res = subprocess.run([sys.executable, RUNNER, "lifecycle", "TransR", str(tmp_path)], capture_output=True, text=True,
-                         timeout=900, cwd=ROOT, env=env)
+                         timeout=900, cwd=ROOT)
     assert res.returncode == 0, res.stdout[-1500:] + res.stderr[-2500:]
     assert "lifecycle ok: TransR" in res.stdout
     assert "avg. triple loss" in res.stdout and "Training ends" in res.stdout
