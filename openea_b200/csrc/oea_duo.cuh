@@ -70,56 +70,6 @@ struct DuoStage {
     float4 Et[4][32];
 };
 
-// Negative sampling of TWO positives by one warp: warp_sample_negatives (oea_sampler.cuh) with lane (half, hl) owning
-// negative hl of its half's positive.  Draw for draw identical to the one-positive routine (the counters use hl, the
-// distinct-position test compares inside a half only), so both kernels sample the same batch from the same seed.
-__device__ __forceinline__ void duo_sample_negatives(const SampledParams& P, uint64_t seed, const oea_kg_view& kg, bool live,
-                                                     int p, int h, int r, int t, int k, int lane,
-                                                     const float* __restrict__ ent_w, int ent_pitch, int& neg_e, bool& neg_head) {
-    const int hl = lane & 15;
-    const uint32_t half_bit = (uint32_t)(lane >> 4) << 31;
-    bool need = live && hl < k;
-    const uint32_t base = rng_base(seed, (uint32_t)P.step, (uint32_t)p);
-    for (int tr = 0; tr < P.max_try; ++tr) {
-        const unsigned missing = __ballot_sync(OEA_FULL, need);
-        if (missing == 0u) break;
-        const bool head = (rng_draw(base, 0x51DEu, tr) >> 31) != 0;  // np.random.binomial(1, .5)
-        const int corrupted = head ? h : t;
-        const int32_t* list = kg.entities;
-        uint32_t C = (uint32_t)kg.n_entities;
-        if (kg.cand != nullptr) {
-            if (kg.ent2row == nullptr) {   // candidate matrix indexed by entity id; a row starting with −1 = no list
-                const int32_t* row = kg.cand + (size_t)corrupted * kg.n_cand;
-                if (__ldg(row) >= 0) { list = row; C = (uint32_t)kg.n_cand; }
-            } else {
-                const int row = __ldg(kg.ent2row + corrupted);
-                if (row >= 0) { list = kg.cand + (size_t)row * kg.n_cand; C = (uint32_t)kg.n_cand; }
-            }
-        }
-        uint32_t pos = 0;
-        bool unsettled = need;
-        for (uint32_t redraw = 0; ; ++redraw) {
-            if (unsettled) pos = bounded32(rng_draw(base, (tr << 8) | hl, 0xC0FFEEu + redraw), C);
-            const unsigned active = __ballot_sync(OEA_FULL, need);
-            unsigned same = 0u;
-            if (need) same = __match_any_sync(active, pos | half_bit);      // C <= 2^31: bit 31 separates the halves
-            unsettled = need && ((same & ((1u << lane) - 1u)) != 0u);
-            if (__ballot_sync(OEA_FULL, unsettled) == 0u) break;
-        }
-        if (need) {
-            const int e = __ldg(list + pos);
-            prefetch_row_l2(ent_w + (size_t)e * ent_pitch, ent_pitch);
-            bool accept = tr == P.max_try - 1;
-            if (!accept) {
-                const uint64_t key = head ? triple_key(e, r, t, P.tset.ent_bits, P.tset.rel_bits)
-                                          : triple_key(h, r, e, P.tset.ent_bits, P.tset.rel_bits);
-                accept = !tset_contains(P.tset, key);
-            }
-            if (accept) { neg_e = e; neg_head = head; need = false; }
-        }
-    }
-}
-
 template <bool FED>
 __device__ __forceinline__ void duo_score_body(const TableDev& ent, const TableDev& rel, const SampledParams& P, const FedBatch& F,
                                                const oea_loss_cfg& cfg, double* __restrict__ loss_out,
@@ -159,29 +109,13 @@ __device__ __forceinline__ void duo_score_body(const TableDev& ent, const TableD
                 neg_general = live && !(share_tail || share_head);
             }
         } else {
-            const int q = p < P.n_slice[0] ? 0 : 1;
-            const oea_kg_view& kg = P.kg[q];
-            const int local = q == 0 ? p : p - P.n_slice[0];
-            const uint32_t tri = (P.diag & 8) ? (uint32_t)(P.start[q] + local)
-                                              : feistel_perm((uint32_t)(P.start[q] + local), (uint32_t)kg.n_triples,
-                                                             seed ^ (q ? 0xA5A5A5A5DEADBEEFull : 0x0123456789ABCDEFull));
-            int hrt = 0;
-            if (hl < 3) hrt = __ldg(kg.triples + 3 * (size_t)tri + hl);
-            h = __shfl_sync(OEA_FULL, hrt, hbase);
-            r = __shfl_sync(OEA_FULL, hrt, hbase + 1);
-            t = __shfl_sync(OEA_FULL, hrt, hbase + 2);
-            if (hl < 3) {   // overlap the three shared rows' fetch with the sampling chain
-                const float* rowp = hl == 1 ? rel.w + (size_t)r * rel.pitch : ent.w + (size_t)(hl == 0 ? h : t) * ent.pitch;
-                prefetch_row_l2(rowp, ent.pitch);
-            }
+            const SampledPositive s = draw_positive<16>(P, seed, p, lane, P.diag & 8, &ent, &rel);
+            const oea_kg_view& kg = P.kg[s.q];
+            h = s.h; r = s.r; t = s.t;
             if (P.diag & 1) { neg_e = __ldg(kg.entities + (uint32_t)(p * 31 + hl * 977) % (uint32_t)kg.n_entities); neg_head = (p + hl) & 1; }
-            else duo_sample_negatives(P, seed, kg, live, p, h, r, t, k, lane, ent.w, ent.pitch, neg_e, neg_head);
+            else sample_negatives<16>(P, seed, kg, live, p, h, r, t, k, lane, ent.w, ent.pitch, neg_e, neg_head);
             const unsigned hm_all = __ballot_sync(OEA_FULL, neg_head);
-            if (dbg != nullptr && live) {
-                int32_t* row = dbg + (size_t)p * (2 + k);
-                if (hl == 0) { row[0] = (int32_t)tri + (q ? (1 << 30) : 0); row[1] = (int32_t)((hm_all >> hbase) & 0xFFFFu); }
-                if (hl < k) row[2 + hl] = neg_e;
-            }
+            if (dbg != nullptr && live) dump_draws<16>(dbg, p, k, s, hm_all, lane, neg_e);
         }
         const unsigned head_mask = __ballot_sync(OEA_FULL, neg_head);
         const unsigned general_mask = FED ? __ballot_sync(OEA_FULL, neg_general) : 0u;

@@ -7,7 +7,7 @@ namespace oea {
 // ------------------------------------------------------------------------------------------------
 // Batch producer (modules/train/batch.py:36-45 / :168-184) for the fed entry points: one warp per positive writes
 // the positive's (h, r, t) and its k negatives as index vectors.  Same positive selection as k_score_sampled.
-// sampler 0: warp_sample_negatives (generate_neg_triples_fast).  sampler 1: generate_neg_triples (batch.py:60-86):
+// sampler 0: sample_negatives<32> (generate_neg_triples_fast).  sampler 1: generate_neg_triples (batch.py:60-86):
 // lane j < k owns negative j, flips its own coin per try, draws one candidate WITH replacement, accepts the first
 // draw that is not a known triple; after max_try rejections the tail becomes a uniform entity of the KG.
 // ------------------------------------------------------------------------------------------------
@@ -22,24 +22,14 @@ k_sample_batch(SampledParams P, int sampler, const float* __restrict__ warm_w, i
     const int k = P.k;
     const size_t n_neg = (size_t)n_pos * k;
     for (int p = warp_global; p < n_pos; p += n_warps) {
-        const int q = p < P.n_slice[0] ? 0 : 1;
-        const oea_kg_view& kg = P.kg[q];
-        const int local = q == 0 ? p : p - P.n_slice[0];
-        const uint32_t tri = feistel_perm((uint32_t)(P.start[q] + local), (uint32_t)kg.n_triples,
-                                          P.seed ^ (q ? 0xA5A5A5A5DEADBEEFull : 0x0123456789ABCDEFull));
-        int hrt = 0;
-        if (lane < 3) {
-            hrt = __ldg(kg.triples + 3 * (size_t)tri + lane);
-            pos_out[(size_t)lane * n_pos + p] = hrt;
-        }
-        const int h = __shfl_sync(OEA_FULL, hrt, 0);
-        const int r = __shfl_sync(OEA_FULL, hrt, 1);
-        const int t = __shfl_sync(OEA_FULL, hrt, 2);
+        const SampledPositive s = draw_positive<32, true>(P, P.seed, p, lane, false, nullptr, nullptr, pos_out, n_pos);
+        const oea_kg_view& kg = P.kg[s.q];
+        const int h = s.h, r = s.r, t = s.t;
         if (k == 0) continue;
         int neg_e = 0;
         bool neg_head = false;
         if (sampler == 0) {
-            warp_sample_negatives(P, P.seed, kg, p, h, r, t, k, lane, warm_w, warm_pitch, neg_e, neg_head);
+            sample_negatives<32>(P, P.seed, kg, true, p, h, r, t, k, lane, warm_w, warm_pitch, neg_e, neg_head);
         } else if (lane < k) {
             const uint32_t base = rng_base(P.seed, (uint32_t)P.step, (uint32_t)p);
             bool done = false;

@@ -1,6 +1,7 @@
 // oea_sampler.cuh — the on-device batch sampler of path (i), shared by the fused step kernels (oea_triple.cu) and the
-// batch producer (oea_sampler.cu): step parameters, the counter RNG, negative sampling of one positive by its warp
-// (modules/train/batch.py:89-119), and the host-side slice arithmetic of batch.py:36-53.  sm_90a.
+// batch producer (oea_sampler.cu): step parameters, the counter RNG, the draw of a positive and its debug-dump row,
+// negative sampling of one positive by a warp or half-warp (modules/train/batch.py:89-119), and the host-side slice
+// arithmetic of batch.py:36-53.  sm_90a.
 #pragma once
 #include <stdlib.h>
 #include "oea_rowmath.cuh"
@@ -31,14 +32,70 @@ __device__ __forceinline__ uint32_t rng_draw(uint32_t base, uint32_t a, uint32_t
     return pcg32(base ^ (a * 0xC2B2AE35u) ^ (b * 0x27D4EB2Fu));
 }
 
-// Negative sampling of one positive by its warp (batch.py:89-119): lane j < k ends up owning negative j
-// (corrupted entity neg_e, neg_head = head corrupted).  Up to max_try rounds; a round flips ONE coin for all
-// still-missing negatives, draws distinct candidate positions for them, keeps the draws that are not known
-// triples; the last round keeps everything.
-__device__ __forceinline__ void warp_sample_negatives(const SampledParams& P, uint64_t seed, const oea_kg_view& kg, int p, int h, int r,
-                                                      int t, int k, int lane, const float* __restrict__ ent_w, int ent_pitch,
-                                                      int& neg_e, bool& neg_head) {
-    bool need = lane < k;
+// Positive p of a sampled step (batch.py:36-53), drawn by a group of LANES lanes: the KG q it comes from, its index
+// `tri` in that KG's triple list (the Feistel permutation of the step's slice, or the slice itself when `identity`) and
+// its (h, r, t), known to every lane of the group.  With `ent` / `rel` given, lanes 0-2 of the group start fetching
+// the three rows into L2, to overlap that fetch with the sampling chain.  With WRITE_POS (the batch producer) they
+// write (h, r, t) to pos_out[hl·n_pos + p].
+struct SampledPositive {
+    int q;
+    uint32_t tri;
+    int h, r, t;
+};
+template <int LANES, bool WRITE_POS = false>
+__device__ __forceinline__ SampledPositive draw_positive(const SampledParams& P, uint64_t seed, int p, int lane, bool identity,
+                                                         const TableDev* ent = nullptr, const TableDev* rel = nullptr,
+                                                         int32_t* __restrict__ pos_out = nullptr, int n_pos = 0) {
+    const int hl = lane & (LANES - 1), hbase = lane & ~(LANES - 1);
+    const int q = p < P.n_slice[0] ? 0 : 1;
+    const oea_kg_view& kg = P.kg[q];
+    const int local = q == 0 ? p : p - P.n_slice[0];
+    const uint32_t tri = identity ? (uint32_t)(P.start[q] + local)
+                                  : feistel_perm((uint32_t)(P.start[q] + local), (uint32_t)kg.n_triples,
+                                                 seed ^ (q ? 0xA5A5A5A5DEADBEEFull : 0x0123456789ABCDEFull));
+    int hrt = 0;
+    if (hl < 3) {
+        hrt = __ldg(kg.triples + 3 * (size_t)tri + hl);
+        if (WRITE_POS) pos_out[(size_t)hl * n_pos + p] = hrt;
+    }
+    const int h = __shfl_sync(OEA_FULL, hrt, hbase);
+    const int r = __shfl_sync(OEA_FULL, hrt, hbase + 1);
+    const int t = __shfl_sync(OEA_FULL, hrt, hbase + 2);
+    if (ent != nullptr && hl < 3) {
+        const float* rowp = hl == 1 ? rel->w + (size_t)r * rel->pitch : ent->w + (size_t)(hl == 0 ? h : t) * ent->pitch;
+        prefetch_row_l2(rowp, ent->pitch);
+    }
+    return SampledPositive{q, tri, h, r, t};
+}
+
+// Row p of the optional debug dump of a sampled step: the triple index with bit 30 set for KG 2, the group's head
+// mask (bit j: negative j corrupts the head; `head_mask` is the warp's ballot) and the k negatives.
+template <int LANES>
+__device__ __forceinline__ void dump_draws(int32_t* __restrict__ dbg, int p, int k, const SampledPositive& s, unsigned head_mask,
+                                           int lane, int neg_e) {
+    const int hl = lane & (LANES - 1), hbase = lane & ~(LANES - 1);
+    int32_t* row = dbg + (size_t)p * (2 + k);
+    if (hl == 0) {
+        row[0] = (int32_t)s.tri + (s.q ? (1 << 30) : 0);
+        row[1] = (int32_t)(LANES == 32 ? head_mask : (head_mask >> hbase) & ((1u << LANES) - 1u));
+    }
+    if (hl < k) row[2 + hl] = neg_e;
+}
+
+// Negative sampling of one positive by a group of LANES lanes (a warp, or a half-warp of the duo scorer)
+// (batch.py:89-119): lane hl < k of the group ends up owning negative hl (corrupted entity neg_e, neg_head = head
+// corrupted).  Up to max_try rounds; a round flips ONE coin for all still-missing negatives, draws distinct candidate
+// positions for them, keeps the draws that are not known triples; the last round keeps everything.  The counters use
+// hl and the distinct-position test compares inside a group only, so a half-warp draws exactly what a warp draws for
+// the same positive and seed.  A group that is not `live` samples nothing.
+template <int LANES>
+__device__ __forceinline__ void sample_negatives(const SampledParams& P, uint64_t seed, const oea_kg_view& kg, bool live, int p,
+                                                 int h, int r, int t, int k, int lane, const float* __restrict__ ent_w,
+                                                 int ent_pitch, int& neg_e, bool& neg_head) {
+    static_assert(LANES == 16 || LANES == 32, "a warp or a half-warp");
+    const int hl = lane & (LANES - 1);
+    const uint32_t group_bit = (uint32_t)(lane / LANES) << 31;   // C <= 2^31: bit 31 separates the half-warps
+    bool need = live && hl < k;
     const uint32_t base = rng_base(seed, (uint32_t)P.step, (uint32_t)p);
     for (int tr = 0; tr < P.max_try; ++tr) {
         const unsigned missing = __ballot_sync(OEA_FULL, need);
@@ -60,10 +117,10 @@ __device__ __forceinline__ void warp_sample_negatives(const SampledParams& P, ui
         uint32_t pos = 0;
         bool unsettled = need;
         for (uint32_t redraw = 0; ; ++redraw) {
-            if (unsettled) pos = bounded32(rng_draw(base, (tr << 8) | lane, 0xC0FFEEu + redraw), C);
+            if (unsettled) pos = bounded32(rng_draw(base, (tr << 8) | hl, 0xC0FFEEu + redraw), C);
             const unsigned active = __ballot_sync(OEA_FULL, need);
             unsigned same = 0u;
-            if (need) same = __match_any_sync(active, pos);
+            if (need) same = __match_any_sync(active, pos | group_bit);
             // the lowest lane of a duplicate group keeps its draw, the others redraw
             unsettled = need && ((same & ((1u << lane) - 1u)) != 0u);
             if (__ballot_sync(OEA_FULL, unsettled) == 0u) break;

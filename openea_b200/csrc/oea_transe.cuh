@@ -69,7 +69,7 @@ struct FedBatch {
 // l2_normalize is linear in the incoming gradient) and leave as three vector reductions per positive: 3 + k row loads
 // and 3 + k row reductions per positive instead of 3·(1 + k) each.
 //   SAMPLED (FED = false): the positive is drawn by the Feistel permutation of the step's slice and its negatives by
-//     warp_sample_negatives (modules/train/batch.py:89-119); `dbg` (optional) receives the draws.
+//     sample_negatives<32> (oea_sampler.cuh, modules/train/batch.py:89-119); `dbg` (optional) receives the draws.
 //   FED: positive p and negatives p·k + j from F.  A negative that shares fewer than two rows with its positive (any
 //     fed batch is legal) is scored as a general triple.
 template <int SCORE, int VEC, bool FED>
@@ -95,29 +95,13 @@ __device__ __forceinline__ void positive_score_body(const TableDev& ent, const T
         if (FED) {
             h = __ldg(F.ph + p); r = __ldg(F.pr + p); t = __ldg(F.pt + p);
         } else {
-            const int q = p < P.n_slice[0] ? 0 : 1;
-            const oea_kg_view& kg = P.kg[q];
-            const int local = q == 0 ? p : p - P.n_slice[0];
-            const uint32_t tri = feistel_perm((uint32_t)(P.start[q] + local), (uint32_t)kg.n_triples,
-                                              seed ^ (q ? 0xA5A5A5A5DEADBEEFull : 0x0123456789ABCDEFull));
-            int hrt = 0;
-            if (lane < 3) hrt = __ldg(kg.triples + 3 * (size_t)tri + lane);
-            h = __shfl_sync(OEA_FULL, hrt, 0);
-            r = __shfl_sync(OEA_FULL, hrt, 1);
-            t = __shfl_sync(OEA_FULL, hrt, 2);
-            if (lane < 3) {   // overlap the three shared rows' fetch with the sampling chain
-                const float* rowp = lane == 1 ? rel.w + (size_t)r * rel.pitch : ent.w + (size_t)(lane == 0 ? h : t) * ent.pitch;
-                prefetch_row_l2(rowp, ent.pitch);
-            }
+            const SampledPositive s = draw_positive<32>(P, seed, p, lane, false, &ent, &rel);
+            h = s.h; r = s.r; t = s.t;
             // lane j < k owns negative j
             bool neg_head = false;
-            warp_sample_negatives(P, seed, kg, p, h, r, t, k, lane, ent.w, ent.pitch, neg_e, neg_head);
+            sample_negatives<32>(P, seed, P.kg[s.q], true, p, h, r, t, k, lane, ent.w, ent.pitch, neg_e, neg_head);
             head_mask = __ballot_sync(OEA_FULL, neg_head);
-            if (dbg != nullptr) {
-                int32_t* row = dbg + (size_t)p * (2 + k);
-                if (lane == 0) { row[0] = (int32_t)tri + (q ? (1 << 30) : 0); row[1] = (int32_t)head_mask; }
-                if (lane < k) row[2 + lane] = neg_e;
-            }
+            if (dbg != nullptr) dump_draws<32>(dbg, p, k, s, head_mask, lane, neg_e);
         }
 
         // ---- positive triple ----

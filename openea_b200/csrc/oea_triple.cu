@@ -73,32 +73,16 @@ __device__ __forceinline__ void oct_score_body(const TableDev& ent, const TableD
     float lane_loss = 0.f;
 
     for (int p = warp_global * P.shard_world + P.shard_rank; p < n_pos; p += n_warps * P.shard_world) {
-        const int q = p < P.n_slice[0] ? 0 : 1;
-        const oea_kg_view& kg = P.kg[q];
-        const int local = q == 0 ? p : p - P.n_slice[0];
-        const uint32_t tri = (P.diag & 8) ? (uint32_t)(P.start[q] + local)
-                                          : feistel_perm((uint32_t)(P.start[q] + local), (uint32_t)kg.n_triples,
-                                                         seed ^ (q ? 0xA5A5A5A5DEADBEEFull : 0x0123456789ABCDEFull));
-        int hrt = 0;
-        if (lane < 3) hrt = __ldg(kg.triples + 3 * (size_t)tri + lane);
-        const int h = __shfl_sync(OEA_FULL, hrt, 0);
-        const int r = __shfl_sync(OEA_FULL, hrt, 1);
-        const int t = __shfl_sync(OEA_FULL, hrt, 2);
-        if (lane < 3) {   // overlap the three shared rows' fetch with the sampling chain
-            const float* rowp = lane == 1 ? rel.w + (size_t)r * rel.pitch : ent.w + (size_t)(lane == 0 ? h : t) * ent.pitch;
-            prefetch_row_l2(rowp, ent.pitch);
-        }
+        const SampledPositive s = draw_positive<32>(P, seed, p, lane, P.diag & 8, &ent, &rel);
+        const oea_kg_view& kg = P.kg[s.q];
+        const int h = s.h, r = s.r, t = s.t;
 
         int neg_e = 0;
         bool neg_head = false;
         if (P.diag & 1) { neg_e = __ldg(kg.entities + (uint32_t)(p * 31 + lane * 977) % (uint32_t)kg.n_entities); neg_head = (p + lane) & 1; }
-        else warp_sample_negatives(P, seed, kg, p, h, r, t, k, lane, ent.w, ent.pitch, neg_e, neg_head);
+        else sample_negatives<32>(P, seed, kg, true, p, h, r, t, k, lane, ent.w, ent.pitch, neg_e, neg_head);
         const unsigned head_mask = __ballot_sync(OEA_FULL, neg_head);
-        if (dbg != nullptr) {
-            int32_t* row = dbg + (size_t)p * (2 + k);
-            if (lane == 0) { row[0] = (int32_t)tri + (q ? (1 << 30) : 0); row[1] = (int32_t)head_mask; }
-            if (lane < k) row[2 + lane] = neg_e;
-        }
+        if (dbg != nullptr) dump_draws<32>(dbg, p, k, s, head_mask, lane, neg_e);
 
         // ---- phase 1: the three shared rows (every octet computes the same copy; octet 0 stages it) ----
         float ih, ir, it, ssh, ssr, sst, sp;

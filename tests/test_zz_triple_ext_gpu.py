@@ -218,7 +218,7 @@ def test_batch_producer_properties(cuda_device, sampler, k):
 
 
 def test_fast_batch_producer_draws_the_same_negatives_as_the_fused_kernel(cuda_device):
-    """sampler 0 shares warp_sample_negatives and the positive permutation with k_score_sampled: for one seed the
+    """sampler 0 shares sample_negatives<32> and draw_positive (oea_sampler.cuh) with k_score_sampled: for one seed the
     index vectors equal the fused kernel's debug dump (the L1 score: the warp-per-positive kernel)."""
     eng = _engine()
     rng = np.random.default_rng(23)
