@@ -100,6 +100,10 @@ typedef struct oea_tripleset {
     uint32_t        capacity; /* power of two */
     uint32_t        ent_bits; /* key = (h << (ent_bits + rel_bits)) | (r << ent_bits) | t */
     uint32_t        rel_bits;
+    const uint64_t* filter;   /* optional blocked Bloom filter of the same keys [filter_words] (one word and four bits
+                               * per key, tset_filter_hash / tset_filter_bits of oea_common.cuh), or NULL: a key the
+                               * filter rejects is absent without probing `slots` */
+    uint32_t        filter_words; /* power of two when filter != NULL */
 } oea_tripleset;
 
 typedef struct oea_sample_cfg {

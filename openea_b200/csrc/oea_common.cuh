@@ -204,7 +204,24 @@ __host__ __device__ __forceinline__ uint32_t key_hash(uint64_t key) {
 __host__ __device__ __forceinline__ uint64_t triple_key(uint32_t h, uint32_t r, uint32_t t, uint32_t ent_bits, uint32_t rel_bits) {
     return ((uint64_t)h << (ent_bits + rel_bits)) | ((uint64_t)r << ent_bits) | (uint64_t)t;
 }
+// Blocked Bloom filter in front of the slots: a key sets four bits of ONE 64-bit word.  The word comes from a hash
+// independent of key_hash (high and low halves swap roles), so a key's slot and its filter word are uncorrelated; the
+// four bit positions are four 6-bit fields of one further mix of that hash.  engine.tripleset_filter restates both in
+// torch.  At ≥ 16 bits per key the filter rejects ≈ 99 % of absent keys with one load from a table 8× smaller than the
+// slots (2 MB at the 100K shape), which stays in L2 where the slots do not.
+__host__ __device__ __forceinline__ uint32_t tset_filter_hash(uint64_t key) {
+    return pcg32((uint32_t)(key >> 32) ^ pcg32((uint32_t)key ^ 0x2545F491u));
+}
+__host__ __device__ __forceinline__ uint64_t tset_filter_bits(uint32_t fh) {
+    const uint32_t b = pcg32(fh ^ 0x68E31DA4u);
+    return (1ull << (b & 63u)) | (1ull << ((b >> 6) & 63u)) | (1ull << ((b >> 12) & 63u)) | (1ull << ((b >> 18) & 63u));
+}
 __device__ __forceinline__ bool tset_contains(const oea_tripleset& s, uint64_t key) {
+    if (s.filter != nullptr) {
+        const uint32_t fh = tset_filter_hash(key);
+        const uint64_t bits = tset_filter_bits(fh);
+        if ((__ldg(s.filter + (fh & (s.filter_words - 1u))) & bits) != bits) return false;
+    }
     const uint32_t mask = s.capacity - 1u;
     uint32_t slot = key_hash(key) & mask;
     while (true) {

@@ -167,6 +167,7 @@ inline int sampler_prepare(const oea_kg_view* kg1, const oea_kg_view* kg2, const
     if (!smp || !tset || !tset->slots) return OEA_ERR_NULL;
     if (smp->neg_per_pos < 0 || smp->neg_per_pos > 32 || smp->batch_size < 1 || smp->max_try < 1 || smp->step < 0) return OEA_ERR_RANGE;
     if (tset->capacity == 0 || (tset->capacity & (tset->capacity - 1)) != 0) return OEA_ERR_RANGE;
+    if (tset->filter && (tset->filter_words == 0 || (tset->filter_words & (tset->filter_words - 1)) != 0)) return OEA_ERR_RANGE;
     int rc = check_kg(kg1, smp->neg_per_pos); if (rc) return rc;
     rc = check_kg(kg2, smp->neg_per_pos); if (rc) return rc;
     const long long T = (long long)kg1->n_triples + kg2->n_triples;

@@ -201,8 +201,32 @@ class DeviceKG:
                         0 if self.cand is None else self.cand.shape[1])
 
 
+def _pcg32(x):
+    """pcg32 of oea_common.cuh on int64 tensors holding 32-bit values (every product stays below 2^63)."""
+    x = (x * 747796405 + 2891336453) & 0xFFFFFFFF
+    w = (((x >> ((x >> 28) + 4)) ^ x) * 277803737) & 0xFFFFFFFF
+    return (w >> 22) ^ w
+
+
+def tripleset_filter(slots):
+    """The blocked Bloom filter of the keys held in `slots` (int64, empty = -1): int64 words, a power of two of them
+    and at least 16 bits per key.  Restates tset_filter_hash / tset_filter_bits of oea_common.cuh: a key sets four
+    bits of one word."""
+    keys = slots[slots != -1]
+    n_words = 1 << (max(1, (keys.numel() + 3) // 4) - 1).bit_length()
+    fh = _pcg32((keys >> 32) ^ _pcg32((keys & 0xFFFFFFFF) ^ 0x2545F491))
+    b = _pcg32(fh ^ 0x68E31DA4)
+    word = (fh & (n_words - 1)) * 64
+    bitmap = torch.zeros(n_words * 64, dtype=torch.bool, device=slots.device)
+    for shift in (0, 6, 12, 18):
+        bitmap[word + ((b >> shift) & 63)] = True
+    weights = torch.ones(64, dtype=torch.int64, device=slots.device) << torch.arange(64, device=slots.device)
+    return (bitmap.view(n_words, 64).to(torch.int64) * weights).sum(1)
+
+
 class DeviceTripleSet:
-    """Open-addressing membership set of (h, r, t) built on device (oea_tripleset_build)."""
+    """Open-addressing membership set of (h, r, t) built on device (oea_tripleset_build), with the blocked Bloom
+    filter that answers most "absent" queries from L2 (tripleset_filter)."""
 
     def __init__(self, triple_tensors, n_ent, n_rel, device="cuda"):
         lib = L.load()
@@ -216,9 +240,11 @@ class DeviceTripleSet:
         self.capacity = cap
         L.check(lib.oea_tripleset_build(_ptr(allt), n, _ptr(self.slots), cap, self.ent_bits, self.rel_bits,
                                         _stream_ptr()), "oea_tripleset_build")
+        self.filter = tripleset_filter(self.slots)
 
     def view(self):
-        return L.TripleSet(self.slots.data_ptr(), self.capacity, self.ent_bits, self.rel_bits)
+        return L.TripleSet(self.slots.data_ptr(), self.capacity, self.ent_bits, self.rel_bits, self.filter.data_ptr(),
+                           self.filter.numel())
 
 
 class TripleTrainer:

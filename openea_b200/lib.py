@@ -46,7 +46,8 @@ class KgView(C.Structure):
 
 
 class TripleSet(C.Structure):
-    _fields_ = [("slots", C.c_void_p), ("capacity", C.c_uint32), ("ent_bits", C.c_uint32), ("rel_bits", C.c_uint32)]
+    _fields_ = [("slots", C.c_void_p), ("capacity", C.c_uint32), ("ent_bits", C.c_uint32), ("rel_bits", C.c_uint32),
+                ("filter", C.c_void_p), ("filter_words", C.c_uint32)]
 
 
 class SampleCfg(C.Structure):
