@@ -341,6 +341,37 @@ int oea_proje_score_fed(const oea_proje* model, const int32_t* pos_h, const int3
                         int32_t n_pos, const int32_t* sampled, const int32_t* num_tries, int32_t num_sampled,
                         void* workspace, size_t workspace_bytes, double* loss_out, void* stream);
 
+/* ---- path (i), the general sampled-NCE step (approaches/attr2vec.py) ---------------------------------------------- */
+
+/* The variables of tf.nn.nce_loss applied to an embedding lookup.  in and cls_w share dim and a pitch <= 128; each is
+ * looked up through l2_normalize when its own l2_norm is set (Attr2Vec: both, xavier_init(…, True)).  cls_b: the
+ * biases stored as [C, 1], raw. */
+typedef struct oea_nce {
+    const oea_table* in;
+    const oea_table* cls_w;
+    const oea_table* cls_b;
+} oea_nce;
+
+/* loss = loss_scale · Σ_b tf.nn.nce_loss(ŵ, cls_b, label = labels[b], x̂ = in[inputs[b]]) over the given sampled set of
+ * oea_logu_sample_unique (the whole batch shares it): logits x̂·ŵ_c + b_c − log q(c) as oea_proje_score_fed, sigmoid
+ * cross-entropy, accidental hits kept.  Attr2Vec's reduce_mean is loss_scale = 1/n (attr2vec.py:121-123).
+ * *loss_out (device fp64) += loss; the three tables' grad += loss_scale · d loss / d raw variable, touched rows flagged.
+ * FP32 throughout.  OEA_ERR_DIM when the pitch exceeds 128 or in and cls_w disagree in dim or pitch; OEA_ERR_SHAPE when
+ * cls_b is not [cls_w->rows, 1]; OEA_ERR_RANGE unless 1 <= num_sampled <= cls_w->rows; OEA_ERR_WORKSPACE when the
+ * 16-byte aligned workspace is smaller than oea_nce_workspace_bytes(n, num_sampled, dim, cls_w->rows), which also
+ * covers oea_logu_sample_unique over cls_w->rows classes.  Run oea_rowopt_apply on the three tables afterwards. */
+size_t oea_nce_workspace_bytes(int32_t n, int32_t num_sampled, int32_t dim, int32_t n_classes);
+int oea_nce_score_fed(const oea_nce* model, const int32_t* inputs, const int32_t* labels, int32_t n,
+                      const int32_t* sampled, const int32_t* num_tries, int32_t num_sampled, float loss_scale,
+                      void* workspace, size_t workspace_bytes, double* loss_out, void* stream);
+
+/* random.sample(pairs, batch) of attr2vec.py:150 on the device: first[i], second[i] = pairs[2·r_i], pairs[2·r_i + 1]
+ * for r_i = feistel_perm(i, n_pairs, key(seed, epoch, step)), i < batch — a keyed permutation of the rows restricted to
+ * its first `batch` positions, so the rows are distinct within a call; it is not a uniformly random subset.
+ * pairs: device int32 [n_pairs, 2].  OEA_ERR_RANGE unless 0 <= batch <= n_pairs. */
+int oea_pairs_draw(const int32_t* pairs, int32_t n_pairs, int32_t batch, uint64_t seed, int32_t epoch, int32_t step,
+                   int32_t* first, int32_t* second, void* stream);
+
 /* The batch producer of modules/train/batch.py:36-45 (generate_relation_triple_batch) / :168-184
  * (generate_triple_label_batch) on the device: writes the index vectors a fed step takes.
  *   pos_hrt [3, n_pos] (h | r | t rows), neg_hrt [3, n_pos·neg_per_pos] (negatives of positive p at p·k … p·k+k−1),

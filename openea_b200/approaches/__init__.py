@@ -1,4 +1,5 @@
 from openea_b200.approaches.aligne import AlignE
+from openea_b200.approaches.attr2vec import Attr2Vec
 from openea_b200.approaches.attre import AttrE
 from openea_b200.approaches.bootea import BootEA
 from openea_b200.approaches.bootea_rotate import BootEA_RotatE
@@ -13,7 +14,6 @@ from openea_b200.approaches.alinet import AliNet
 from openea_b200.approaches.gcn_align import GCN_Align
 from openea_b200.approaches.rdgcn import RDGCN
 
-Attr2Vec = out_of_scope("Attr2Vec", "stand-alone attribute skip-gram model (JAPE carries its own auxiliary, approaches/jape.py)")
 RSN4EA = out_of_scope("RSN4EA", "recurrent skipping network over paths")
 MultiKE = out_of_scope("MultiKE", "multi-view literal/attribute encoders")
 GMNN = out_of_scope("GMNN", "graph matching network")

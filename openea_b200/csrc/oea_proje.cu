@@ -1,6 +1,8 @@
 // oea_proje.cu — path (i), ProjE: TF's unique log-uniform candidate sampler on the device and the step of
 // models/neural/proje.py:46-74 (a projection layer with three training-mode batch norms, then tf.nn.nce_loss over one
-// sampled set of classes the whole batch shares).  sm_90a, FP32 FFMA only.
+// sampled set of classes the whole batch shares).  The same sampler and NCE head also make the general sampled-NCE step
+// of approaches/attr2vec.py:113-124 (oea_nce_score_fed) and its per-step pair draw (oea_pairs_draw).
+// sm_90a, FP32 FFMA only.
 //
 // Maths restated from the reference and from TF 1.x (no code shared):
 //   models/neural/proje.py:51-62   x_h = ê[h], x_r = r̂[r]; y_h = BN(x_h), y_r = BN(x_r) with ONE shared beta and each its
@@ -32,6 +34,21 @@
 //   7. k_proje_columns_bwd  one CTA per column: back through the three BNs and the combination; the gradients of mlp_w,
 //                           mlp_bias and both betas are this CTA's column sums
 //   8. k_proje_push         one warp per positive: dx_h, dx_r through the tables' normalisation into ent.grad, rel.grad
+//
+// oea_nce_score_fed: loss_scale · Σ_b nce_loss(ŵ, b, label_b, x̂[input_b]) with each table normalised or raw by its own
+// flag.  A memset and nine kernels, the head's three GEMMs shared with ProjE through the W_S addressing policy:
+//   1. k_nce_stage          one warp per sampled class: ŵ_s and its 1/‖w_s‖, Σw² into the workspace ([S, pitch],
+//                           contiguous), dŴ_s zeroed
+//   2. k_nce_gather         one warp per row of the batch: x̂[input_b] into the workspace
+//   3. k_nce_logq, k_nce_logits<StagedW>, k_nce_dx<StagedW>, k_nce_dw<StagedW>: the head over the staged block; G
+//                           carries the scale, dŴ_S accumulates in the workspace
+//   4. k_nce_true           one warp per row: ŵ_label normalised in registers, the true logit, its loss, dX, and its
+//                           part of the label row's gradient pushed through the normalisation itself
+//   5. k_nce_w_push         one warp per sampled class: dŴ_s through the normalisation into cls_w.grad (red: a sampled
+//                           class can also be a label; the Jacobian is linear, so the two parts are pushed separately)
+//   6. k_nce_in_push        one warp per row: dX through the input table's normalisation into its gradient
+//
+// oea_pairs_draw: B distinct rows of an [n, 2] pair array, row i = feistel_perm(i, n, key(seed, epoch, step)) for i < B.
 #include "oea_rowmath.cuh"
 
 namespace oea {
@@ -156,6 +173,32 @@ __device__ __forceinline__ float sigmoid_acc(float x) { return 1.f / (1.f + expf
 struct ProjeDev {
     TableDev ent, rel, w, b, prm;
     int dim, pitch, n_classes, num_sampled, ldg;
+};
+
+// How the NCE head addresses the sampled classes' rows W_S and scales its loss (the last kernel argument).  The row of
+// sampled slot s is asked for with `id` = sampled + s, written as the kernel always wrote it (ProjE's SASS depends on
+// that address arithmetic), and with s itself.  ProjE: entity_w rows gathered by class id, dW_S reduced straight into
+// entity_w's gradient, the loss summed.
+struct GatheredW {
+    __device__ __forceinline__ const float* w_row(const ProjeDev& T, const int32_t* id, int) const {
+        return T.w.w + (size_t)__ldg(id) * T.pitch;
+    }
+    __device__ __forceinline__ float* dw_row(const ProjeDev& T, const int32_t* id, int) const {
+        return T.w.g + (size_t)__ldg(id) * T.pitch;
+    }
+    __device__ __forceinline__ float scaled(float v) const { return v; }
+};
+// oea_nce_score_fed: ŵ_S staged contiguously by k_nce_stage, dŴ_S accumulated in the workspace (k_nce_w_push takes it
+// through the normalisation), loss and every gradient times `scale`
+struct StagedW {
+    const float* w;
+    float* dw;
+    float scale;
+    __device__ __forceinline__ const float* w_row(const ProjeDev& T, const int32_t*, int s) const {
+        return w + (size_t)s * T.pitch;
+    }
+    __device__ __forceinline__ float* dw_row(const ProjeDev& T, const int32_t*, int s) const { return dw + (size_t)s * T.pitch; }
+    __device__ __forceinline__ float scaled(float v) const { return v * scale; }
 };
 
 // ---- projection layer ----------------------------------------------------------------------------------------------
@@ -354,9 +397,10 @@ __device__ __forceinline__ void zero_acc(float (&acc)[8][8]) {
 }
 
 // logits of the sampled classes: tile (bt, st) of [n × S]; G = σ(logit) for the backward, Σ_b G into entity_b's gradient
+template <class H>
 __global__ void __launch_bounds__(kThreads)
 k_nce_logits(ProjeDev T, int n, const float* __restrict__ x, const int32_t* __restrict__ sampled,
-             const float* __restrict__ lqs, float* __restrict__ G, double* __restrict__ loss_out) {
+             const float* __restrict__ lqs, float* __restrict__ G, double* __restrict__ loss_out, H h) {
     __shared__ __align__(16) float As[kTk * kTld];
     __shared__ __align__(16) float Bs[kTk * kTld];
     __shared__ float s_db[kTile];
@@ -372,8 +416,7 @@ k_nce_logits(ProjeDev T, int n, const float* __restrict__ x, const int32_t* __re
         for (int k0 = 0; k0 < T.pitch; k0 += kTk) {
             __syncthreads();
             stage_rows_t(As, [&](int i) { return m0 + i < n ? x + (size_t)(m0 + i) * T.pitch : nullptr; }, k0, T.pitch);
-            stage_rows_t(Bs, [&](int i) { return n0 + i < S ? T.w.w + (size_t)__ldg(sampled + n0 + i) * T.pitch : nullptr; },
-                         k0, T.pitch);
+            stage_rows_t(Bs, [&](int i) { return n0 + i < S ? h.w_row(T, sampled + n0 + i, n0 + i) : nullptr; }, k0, T.pitch);
             __syncthreads();
             tile_mma(acc, As, Bs, ty, tx);
         }
@@ -397,7 +440,7 @@ k_nce_logits(ProjeDev T, int n, const float* __restrict__ x, const int32_t* __re
                 if (s < S) {
                     const float logit = acc[a][b] + bias - lq;
                     lsum += softplus(logit);
-                    g = sigmoid_acc(logit);
+                    g = h.scaled(sigmoid_acc(logit));
                     col += g;
                 }
                 G[(size_t)m * T.ldg + s] = g;
@@ -412,13 +455,14 @@ k_nce_logits(ProjeDev T, int n, const float* __restrict__ x, const int32_t* __re
         }
     }
     LossAcc lacc{s_loss};
-    lacc.flush(warp_sum(lsum), loss_out);
+    lacc.flush(h.scaled(warp_sum(lsum)), loss_out);
 }
 
 // dX[b][:] += Σ_{s in split} G[b][s]·W_S[s][:]; tile t = (b tile, split of the sampled set)
+template <class H>
 __global__ void __launch_bounds__(kThreads)
 k_nce_dx(ProjeDev T, int n, const float* __restrict__ G, const int32_t* __restrict__ sampled, int split,
-         float* __restrict__ dx) {
+         float* __restrict__ dx, H h) {
     __shared__ __align__(16) float As[kTk * kTld];
     __shared__ __align__(16) float Bs[kTk * kTld];
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
@@ -434,8 +478,7 @@ k_nce_dx(ProjeDev T, int n, const float* __restrict__ G, const int32_t* __restri
             // are zero, so the slice needs no clipping inside a float4
             stage_rows_t(As, [&](int i) { return m0 + i < n ? G + (size_t)(m0 + i) * T.ldg : nullptr; }, k0,
                          (s1 + 3) / 4 * 4);
-            stage_rows_n(Bs, [&](int k) { return k0 + k < s1 ? T.w.w + (size_t)__ldg(sampled + k0 + k) * T.pitch : nullptr; },
-                         T.pitch);
+            stage_rows_n(Bs, [&](int k) { return k0 + k < s1 ? h.w_row(T, sampled + k0 + k, k0 + k) : nullptr; }, T.pitch);
             __syncthreads();
             tile_mma(acc, As, Bs, ty, tx);
         }
@@ -452,10 +495,11 @@ k_nce_dx(ProjeDev T, int n, const float* __restrict__ G, const int32_t* __restri
     }
 }
 
-// entity_w.grad[sampled[s]][:] += Σ_{b in split} G[b][s]·X[b][:]; tile t = (sampled tile, split of the batch)
+// dW_S[s][:] += Σ_{b in split} G[b][s]·X[b][:]; tile t = (sampled tile, split of the batch)
+template <class H>
 __global__ void __launch_bounds__(kThreads)
 k_nce_dw(ProjeDev T, int n, const float* __restrict__ G, const float* __restrict__ x, const int32_t* __restrict__ sampled,
-         int split) {
+         int split, H h) {
     __shared__ __align__(16) float As[kTk * kTld];
     __shared__ __align__(16) float Bs[kTk * kTld];
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
@@ -485,8 +529,7 @@ k_nce_dw(ProjeDev T, int n, const float* __restrict__ G, const float* __restrict
             for (int e = threadIdx.x; e < 16 * (kTile / 4); e += blockDim.x) {
                 const int r = e >> 5, c = 4 * (e & 31), s = m0 + r + 16 * a;
                 if (s < S && c < T.pitch)
-                    red_add4(T.w.g + (size_t)__ldg(sampled + s) * T.pitch + c,
-                             *reinterpret_cast<const float4*>(Cs + r * kTld + c));
+                    red_add4(h.dw_row(T, sampled + s, s) + c, *reinterpret_cast<const float4*>(Cs + r * kTld + c));
             }
             __syncthreads();
         }
@@ -523,6 +566,151 @@ k_proje_true(ProjeDev T, const int32_t* __restrict__ pt, int n, const float* __r
     }
     LossAcc lacc{s_loss};
     lacc.flush(warp_sum(lsum), loss_out);
+}
+
+// ---- the general sampled-NCE step (oea_nce_score_fed) ---------------------------------------------------------------
+struct NceWs {
+    size_t first, x, dx, w, dw, winv, wss, lq, g, total;
+    int ldg;
+};
+
+// workspace sections, each 256-B aligned: the sampler's first-draw index per class, x̂ and dX̂ [n, pitch], ŵ_S and dŴ_S
+// [S, pitch], 1/‖w_s‖ and Σw_s² [S], log q [S], G [n, ldg]
+static NceWs nce_layout(int n, int num_sampled, int pitch, int n_classes) {
+    NceWs w;
+    size_t at = 0;
+    auto take = [&](size_t bytes) { const size_t o = at; at += (bytes + 255) & ~(size_t)255; return o; };
+    w.ldg = (num_sampled + 3) / 4 * 4;
+    w.first = take(4 * (size_t)n_classes);
+    w.x = take(4 * (size_t)n * pitch);
+    w.dx = take(4 * (size_t)n * pitch);
+    w.w = take(4 * (size_t)num_sampled * pitch);
+    w.dw = take(4 * (size_t)num_sampled * pitch);
+    w.winv = take(4 * (size_t)num_sampled);
+    w.wss = take(4 * (size_t)num_sampled);
+    w.lq = take(4 * (size_t)num_sampled);
+    w.g = take(4 * (size_t)n * w.ldg);
+    w.total = at;
+    return w;
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_nce_stage(ProjeDev T, const int32_t* __restrict__ sampled, float* __restrict__ ws_w, float* __restrict__ ws_dw,
+            float* __restrict__ winv, float* __restrict__ wss) {
+    const int lane = threadIdx.x & 31;
+    for (int s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; s < T.num_sampled; s += (gridDim.x * blockDim.x) >> 5) {
+        const NRow<1> w = lookup<1>(T.w, __ldg(sampled + s), lane);
+        if (4 * lane < T.pitch) {
+            *reinterpret_cast<float4*>(ws_w + (size_t)s * T.pitch + 4 * lane) = w.x.v[0];
+            *reinterpret_cast<float4*>(ws_dw + (size_t)s * T.pitch + 4 * lane) = f4(0.f);
+        }
+        if (lane == 0) { winv[s] = w.inv; wss[s] = w.ss; }
+    }
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_nce_gather(ProjeDev T, const int32_t* __restrict__ ids, int n, float* __restrict__ x) {
+    const int lane = threadIdx.x & 31;
+    for (int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; b < n; b += (gridDim.x * blockDim.x) >> 5) {
+        const Row<1> v = lookup<1>(T.ent, __ldg(ids + b), lane).x;
+        if (4 * lane < T.pitch) *reinterpret_cast<float4*>(x + (size_t)b * T.pitch + 4 * lane) = v.v[0];
+    }
+}
+
+// the true class of every row: ŵ_label normalised here, the logit, the loss, dX, and the label row's part of its
+// gradient through the normalisation
+__global__ void __launch_bounds__(kThreads)
+k_nce_true(ProjeDev T, const int32_t* __restrict__ labels, int n, const float* __restrict__ x,
+           const int32_t* __restrict__ num_tries, float scale, float* __restrict__ dx, double* __restrict__ loss_out) {
+    __shared__ double s_loss[kWarpsPerBlock];
+    const int lane = threadIdx.x & 31;
+    const int tries = *num_tries;
+    float lsum = 0.f;
+    for (int b0 = (blockIdx.x * blockDim.x) >> 5; b0 < n; b0 += (gridDim.x * blockDim.x) >> 5) {   // warp-uniform
+        const int b = b0 + (threadIdx.x >> 5);
+        if (b >= n) continue;
+        const int c = __ldg(labels + b);
+        const Row<1> xb = load_row<1>(x, b, T.pitch, lane);
+        const NRow<1> wc = lookup<1>(T.w, c, lane);
+        const float logit = warp_sum(dotr(xb, wc.x)) + T.b.w[(size_t)c * T.b.pitch] -
+                            log_expected_count(c, T.n_classes, T.num_sampled, tries);
+        const float g = -sigmoid_acc(-logit) * scale;     // scale·(σ(t) − 1)
+        if (lane == 0) {
+            lsum += softplus(-logit);
+            atomicAdd(T.b.g + (size_t)c * T.b.pitch, g);
+            T.b.touched[c] = 1;
+        }
+        if (4 * lane < T.pitch) {
+            float4* d = reinterpret_cast<float4*>(dx + (size_t)b * T.pitch + 4 * lane);
+            *d = fma4(wc.x.v[0], g, *d);
+        }
+        push<1>(T.w, c, lane, r_scale(xb, g), wc);
+    }
+    LossAcc lacc{s_loss};
+    lacc.flush(warp_sum(lsum) * scale, loss_out);
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_nce_w_push(ProjeDev T, const int32_t* __restrict__ sampled, const float* __restrict__ ws_w,
+             const float* __restrict__ ws_dw, const float* __restrict__ winv, const float* __restrict__ wss) {
+    const int lane = threadIdx.x & 31;
+    for (int s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; s < T.num_sampled; s += (gridDim.x * blockDim.x) >> 5) {
+        NRow<1> w;
+        w.x = load_row<1>(ws_w, s, T.pitch, lane);
+        w.inv = winv[s];
+        w.ss = wss[s];
+        push<1>(T.w, __ldg(sampled + s), lane, load_row<1>(ws_dw, s, T.pitch, lane), w);
+    }
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_nce_in_push(ProjeDev T, const int32_t* __restrict__ ids, int n, const float* __restrict__ dx) {
+    const int lane = threadIdx.x & 31;
+    for (int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; b < n; b += (gridDim.x * blockDim.x) >> 5) {
+        const int i = __ldg(ids + b);
+        push<1>(T.ent, i, lane, load_row<1>(dx, b, T.pitch, lane), lookup<1>(T.ent, i, lane));
+    }
+}
+
+// ---- the per-step pair draw (oea_pairs_draw) ------------------------------------------------------------------------
+__host__ __device__ __forceinline__ uint64_t pairs_key(uint64_t seed, int epoch, int step) {
+    return mix64(seed ^ mix64(((uint64_t)(uint32_t)epoch << 32) | (uint32_t)step));
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_pairs_draw(const int32_t* __restrict__ pairs, uint32_t n, int batch, uint64_t key, int32_t* __restrict__ first,
+             int32_t* __restrict__ second) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < batch; i += gridDim.x * blockDim.x) {
+        const size_t row = feistel_perm((uint32_t)i, n, key);
+        first[i] = __ldg(pairs + 2 * row);
+        second[i] = __ldg(pairs + 2 * row + 1);
+    }
+}
+
+// grids of the head's kernels for a batch of n and S sampled classes
+struct HeadGrids {
+    int rows, lg, dx, dw, split_s, split_b;
+};
+
+static HeadGrids head_grids(int n, int S, int ldg) {
+    HeadGrids h;
+#ifdef OEA_HOST_EMU   // tests/emu: grid-stride kernels on two blocks keep the emulated thread count small
+    h.rows = h.lg = h.dx = h.dw = 2;
+    h.split_s = h.split_b = 2 * kTk;                      // several splits even on small cases
+#else
+    const int mt_b = (n + kTile - 1) / kTile, mt_s = (S + kTile - 1) / kTile;
+    h.rows = grid_for(n);
+    h.lg = mt_b * ((ldg + kTile - 1) / kTile);
+    // split each reduction so that about two CTAs per SM run: a batch of 500 is only four row tiles, and S = 4096
+    // only 32 column tiles.  A split is a multiple of kTk.
+    const int want = 2 * sm_count_cached();
+    auto split_of = [](int len, int parts) { const int s = (len + parts - 1) / parts; return (s + kTk - 1) / kTk * kTk; };
+    h.split_s = split_of(S, (want + mt_b - 1) / mt_b);
+    h.split_b = split_of(n, (want + mt_s - 1) / mt_s);
+    h.dx = mt_b * ((S + h.split_s - 1) / h.split_s);
+    h.dw = mt_s * ((n + h.split_b - 1) / h.split_b);
+#endif
+    return h;
 }
 
 }  // namespace oea
@@ -585,32 +773,95 @@ extern "C" int oea_proje_score_fed(const oea_proje* model, const int32_t* pos_h,
     T.dim = ent->dim; T.pitch = ent->pitch; T.n_classes = w->rows; T.num_sampled = num_sampled; T.ldg = L.ldg;
     cudaStream_t st = (cudaStream_t)stream;
     const int n = n_pos, S = num_sampled;
-#ifdef OEA_HOST_EMU   // tests/emu: grid-stride kernels on two blocks keep the emulated thread count small
-    const int rows_grid = 2, col_grid = 2, lg_grid = 2, dx_grid = 2, dw_grid = 2;
-    const int split_s = 2 * kTk, split_b = 2 * kTk;       // several splits even on small cases
+    const HeadGrids H = head_grids(n, S, L.ldg);
+    const int rows_grid = H.rows;
+#ifdef OEA_HOST_EMU
+    const int col_grid = 2;
 #else
-    const int mt_b = (n + kTile - 1) / kTile, mt_s = (S + kTile - 1) / kTile;
-    const int rows_grid = grid_for(n);
     const int col_grid = ent->pitch;
-    const int lg_grid = mt_b * ((L.ldg + kTile - 1) / kTile);
-    // split each reduction so that about two CTAs per SM run: a batch of 500 is only four row tiles, and S = 4096
-    // only 32 column tiles.  A split is a multiple of kTk.
-    const int want = 2 * sm_count_cached();
-    auto split_of = [](int len, int parts) { const int s = (len + parts - 1) / parts; return (s + kTk - 1) / kTk * kTk; };
-    const int split_s = split_of(S, (want + mt_b - 1) / mt_b), split_b = split_of(n, (want + mt_s - 1) / mt_s);
-    const int dx_grid = mt_b * ((S + split_s - 1) / split_s);
-    const int dw_grid = mt_s * ((n + split_b - 1) / split_b);
 #endif
     OEA_CUDA_TRY(cudaMemsetAsync(dx, 0, 4 * (size_t)n * ent->pitch, st));
     OEA_LAUNCH(k_proje_gather, rows_grid, kThreads, 0, st, T, pos_h, pos_r, n, xh, xr);
     OEA_LAUNCH(k_proje_columns_fwd, col_grid, kThreads, 0, st, T, n, xh, xr, z, x, stats);
     OEA_LAUNCH(k_nce_logq, rows_grid, kThreads, 0, st, sampled, num_tries, T.n_classes, S, lq);
-    OEA_LAUNCH(k_nce_logits, lg_grid, kThreads, 0, st, T, n, x, sampled, lq, G, loss_out);
-    OEA_LAUNCH(k_nce_dx, dx_grid, kThreads, 0, st, T, n, G, sampled, split_s, dx);
-    OEA_LAUNCH(k_nce_dw, dw_grid, kThreads, 0, st, T, n, G, x, sampled, split_b);
+    OEA_LAUNCH(k_nce_logits<GatheredW>, H.lg, kThreads, 0, st, T, n, x, sampled, lq, G, loss_out, GatheredW{});
+    OEA_LAUNCH(k_nce_dx<GatheredW>, H.dx, kThreads, 0, st, T, n, G, sampled, H.split_s, dx, GatheredW{});
+    OEA_LAUNCH(k_nce_dw<GatheredW>, H.dw, kThreads, 0, st, T, n, G, x, sampled, H.split_b, GatheredW{});
     OEA_LAUNCH(k_proje_true, rows_grid, kThreads, 0, st, T, pos_t, n, x, num_tries, dx, loss_out);
     OEA_LAUNCH(k_proje_columns_bwd, col_grid, kThreads, 0, st, T, n, xh, xr, z, dx, stats, dxh, dxr);
     OEA_LAUNCH(k_proje_push, rows_grid, kThreads, 0, st, T, pos_h, pos_r, n, dxh, dxr);
+    OEA_LAUNCH_CHECK();
+    return OEA_OK;
+}
+
+extern "C" size_t oea_nce_workspace_bytes(int32_t n, int32_t num_sampled, int32_t dim, int32_t n_classes) {
+    if (n < 0 || num_sampled < 1 || dim <= 0 || n_classes <= 0) return 0;
+    return nce_layout(n, num_sampled, (dim + 3) / 4 * 4, n_classes).total;
+}
+
+extern "C" int oea_nce_score_fed(const oea_nce* model, const int32_t* inputs, const int32_t* labels, int32_t n,
+                                 const int32_t* sampled, const int32_t* num_tries, int32_t num_sampled, float loss_scale,
+                                 void* workspace, size_t workspace_bytes, double* loss_out, void* stream) {
+    if (model == nullptr) return OEA_ERR_NULL;
+    const oea_table* tabs[3] = {model->in, model->cls_w, model->cls_b};
+    for (const oea_table* t : tabs) {
+        const int rc = check_table(t, true);
+        if (rc) return rc;
+    }
+    const oea_table *in = model->in, *w = model->cls_w, *b = model->cls_b;
+    if (w->dim != in->dim || w->pitch != in->pitch || in->pitch > kProjeMaxPitch) return OEA_ERR_DIM;
+    if (b->rows != w->rows || b->dim != 1) return OEA_ERR_SHAPE;
+    if (num_sampled < 1 || num_sampled > w->rows) return OEA_ERR_RANGE;
+    if (n < 0) return OEA_ERR_SHAPE;
+    if (sampled == nullptr || num_tries == nullptr || loss_out == nullptr) return OEA_ERR_NULL;
+    if (n > 0 && (!inputs || !labels)) return OEA_ERR_NULL;
+    const NceWs L = nce_layout(n, num_sampled, in->pitch, w->rows);
+    if (workspace == nullptr || workspace_bytes < L.total || !aligned16(workspace)) return OEA_ERR_WORKSPACE;
+    if (n == 0) return OEA_OK;
+
+    char* ws = static_cast<char*>(workspace);
+    float* x = reinterpret_cast<float*>(ws + L.x);
+    float* dx = reinterpret_cast<float*>(ws + L.dx);
+    float* ws_w = reinterpret_cast<float*>(ws + L.w);
+    float* ws_dw = reinterpret_cast<float*>(ws + L.dw);
+    float* winv = reinterpret_cast<float*>(ws + L.winv);
+    float* wss = reinterpret_cast<float*>(ws + L.wss);
+    float* lq = reinterpret_cast<float*>(ws + L.lq);
+    float* G = reinterpret_cast<float*>(ws + L.g);
+    ProjeDev T{};
+    T.ent = table_dev(in); T.w = table_dev(w); T.b = table_dev(b);
+    T.b.norm = false;                                     // the biases are a raw [C, 1] variable
+    T.dim = in->dim; T.pitch = in->pitch; T.n_classes = w->rows; T.num_sampled = num_sampled; T.ldg = L.ldg;
+    const StagedW hw{ws_w, ws_dw, loss_scale};
+    cudaStream_t st = (cudaStream_t)stream;
+    const int S = num_sampled;
+    const HeadGrids H = head_grids(n, S, L.ldg);
+#ifdef OEA_HOST_EMU
+    const int s_grid = 2;
+#else
+    const int s_grid = grid_for(S);
+#endif
+    OEA_CUDA_TRY(cudaMemsetAsync(dx, 0, 4 * (size_t)n * in->pitch, st));
+    OEA_LAUNCH(k_nce_stage, s_grid, kThreads, 0, st, T, sampled, ws_w, ws_dw, winv, wss);
+    OEA_LAUNCH(k_nce_gather, H.rows, kThreads, 0, st, T, inputs, n, x);
+    OEA_LAUNCH(k_nce_logq, H.rows, kThreads, 0, st, sampled, num_tries, T.n_classes, S, lq);
+    OEA_LAUNCH(k_nce_logits<StagedW>, H.lg, kThreads, 0, st, T, n, x, sampled, lq, G, loss_out, hw);
+    OEA_LAUNCH(k_nce_dx<StagedW>, H.dx, kThreads, 0, st, T, n, G, sampled, H.split_s, dx, hw);
+    OEA_LAUNCH(k_nce_dw<StagedW>, H.dw, kThreads, 0, st, T, n, G, x, sampled, H.split_b, hw);
+    OEA_LAUNCH(k_nce_true, H.rows, kThreads, 0, st, T, labels, n, x, num_tries, loss_scale, dx, loss_out);
+    OEA_LAUNCH(k_nce_w_push, s_grid, kThreads, 0, st, T, sampled, ws_w, ws_dw, winv, wss);
+    OEA_LAUNCH(k_nce_in_push, H.rows, kThreads, 0, st, T, inputs, n, dx);
+    OEA_LAUNCH_CHECK();
+    return OEA_OK;
+}
+
+extern "C" int oea_pairs_draw(const int32_t* pairs, int32_t n_pairs, int32_t batch, uint64_t seed, int32_t epoch,
+                              int32_t step, int32_t* first, int32_t* second, void* stream) {
+    if (n_pairs < 0 || batch < 0 || batch > n_pairs) return OEA_ERR_RANGE;
+    if (batch == 0) return OEA_OK;
+    if (pairs == nullptr || first == nullptr || second == nullptr) return OEA_ERR_NULL;
+    OEA_LAUNCH_STRIDED(k_pairs_draw, (batch + kThreads - 1) / kThreads, kThreads, 0, (cudaStream_t)stream, pairs,
+                       (uint32_t)n_pairs, batch, pairs_key(seed, epoch, step), first, second);
     OEA_LAUNCH_CHECK();
     return OEA_OK;
 }

@@ -616,6 +616,89 @@ class ProjETrainer:
         return v
 
 
+class NceTrainer:
+    """tf.nn.nce_loss applied to an embedding lookup, one reduce_mean step of approaches/attr2vec.py:113-124,145-161:
+    B distinct pairs drawn on the device (oea_pairs_draw, keyed by (seed, epoch, step)) → TF's unique log-uniform
+    sampler (oea_logu_sample_unique, seeded from the epoch seed and the step as ProjETrainer does) →
+    oea_nce_score_fed with loss_scale 1/B → Adagrad (or the tables' optimiser) on the three tables.
+    tables = (inputs, cls_w, cls_b) EmbeddingTables, cls_b as [C, 1].  Losses accumulate on the device (read_loss)."""
+
+    def __init__(self, tables, num_sampled, lr):
+        self.lib = L.load()
+        self.tables = tuple(tables)
+        self.num_sampled = int(num_sampled)
+        n_classes = self.tables[1].rows
+        if not 1 <= self.num_sampled <= n_classes:
+            raise ValueError("nce_loss samples %d distinct classes out of %d: the sampler's range is too small"
+                             % (self.num_sampled, n_classes))
+        self.lr = float(lr)
+        dev = self.tables[0].device
+        self.loss_dev = torch.zeros(1, dtype=torch.float64, device=dev)
+        self.sampled = torch.zeros(self.num_sampled, dtype=torch.int32, device=dev)
+        self.num_tries = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.pairs = None
+        self._batch = None
+        self._ws = None
+
+    def _workspace(self, n):
+        need = self.lib.oea_nce_workspace_bytes(n, self.num_sampled, self.tables[0].dim, self.tables[1].rows)
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(max(1, need), dtype=torch.uint8, device=self.tables[0].device)
+        return self._ws
+
+    def set_pairs(self, pairs):
+        """The training pairs the steps draw from: [n, 2] (input id, label id), copied to the device once."""
+        self.pairs = torch.as_tensor(np.asarray(pairs, dtype=np.int32).reshape(-1, 2), device=self.tables[0].device)
+
+    def draw(self, batch, seed, epoch, step):
+        """random.sample(pairs, batch) of attr2vec.py:150 as a keyed permutation: (inputs [B], labels [B]) device int32."""
+        if self._batch is None or self._batch.shape[1] < batch:
+            self._batch = torch.empty(2, batch, dtype=torch.int32, device=self.tables[0].device)
+        L.check(self.lib.oea_pairs_draw(_ptr(self.pairs), self.pairs.shape[0], int(batch), int(seed) & (2**64 - 1),
+                                        int(epoch), int(step), _ptr(self._batch[0]), _ptr(self._batch[1]),
+                                        _stream_ptr()), "oea_pairs_draw")
+        return self._batch[0, :batch], self._batch[1, :batch]
+
+    def sample(self, seed):
+        """Draw the step's sampled set into self.sampled / self.num_tries (device; no host synchronisation)."""
+        ws = self._workspace(0)
+        L.check(self.lib.oea_logu_sample_unique(self.tables[1].rows, self.num_sampled, int(seed) & (2**64 - 1),
+                                                _ptr(self.sampled), _ptr(self.num_tries), _ptr(ws), ws.numel(),
+                                                _stream_ptr()), "oea_logu_sample_unique")
+
+    def score_fed(self, inputs, labels, sampled=None, num_tries=None, scale=None, loss_out=None):
+        """inputs / labels: int32 device tensors [n]; sampled / num_tries: int32 device tensors (default: the last
+        sample()); scale: default 1/n (reduce_mean).  Accumulates gradients into the three tables and adds the scaled
+        batch loss into loss_out."""
+        out = self.loss_dev if loss_out is None else loss_out
+        sampled = self.sampled if sampled is None else sampled
+        num_tries = self.num_tries if num_tries is None else num_tries
+        n = inputs.numel()
+        scale = 1.0 / max(1, n) if scale is None else float(scale)
+        ws = self._workspace(n)
+        model = L.Nce(*[C.pointer(t.c_struct()) for t in self.tables])
+        L.check(self.lib.oea_nce_score_fed(C.byref(model), _ptr(inputs), _ptr(labels), n, _ptr(sampled),
+                                           _ptr(num_tries), sampled.numel(), scale, _ptr(ws), ws.numel(), _ptr(out),
+                                           _stream_ptr()), "oea_nce_score_fed")
+
+    def apply(self):
+        for tab in self.tables:
+            tab.apply(self.lr)
+
+    def step(self, batch, seed, epoch, step):
+        """One session.run([loss, optimizer]) of attr2vec.py:156-158 on pairs drawn from set_pairs()."""
+        inputs, labels = self.draw(batch, seed, epoch, step)
+        self.sample(ProjETrainer.step_seed(ProjETrainer.step_seed(seed, epoch), step))
+        self.score_fed(inputs, labels)
+        self.apply()
+
+    def read_loss(self, reset=True):
+        v = float(self.loss_dev.item())
+        if reset:
+            self.loss_dev.zero_()
+        return v
+
+
 class FedHostPipeline:
     """Depth-2 pipeline over TripleTrainer's host-index step (oea_triple_step_fed_host_submit / _collect): the copy of
     step i+1 overlaps the kernels of step i; losses come back one step late.  Owns two streams, four events and the

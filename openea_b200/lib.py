@@ -92,6 +92,11 @@ class Proje(C.Structure):
     _fields_ = [("ent", _TP), ("rel", _TP), ("cls_w", _TP), ("cls_b", _TP), ("params", _TP)]
 
 
+class Nce(C.Structure):
+    # oea_nce: the input table, the class table and the class biases ([C, 1])
+    _fields_ = [("in_", _TP), ("cls_w", _TP), ("cls_b", _TP)]
+
+
 class Model(C.Structure):
     # gamma / phase: RotatE's model constants (0 and ignored for the other kinds)
     _fields_ = [("kind", C.c_int32), ("ent", _TP), ("rel", _TP), ("ent_aux", _TP), ("rel_aux", _TP),
@@ -158,6 +163,9 @@ SIGNATURES = {
     "oea_logu_sample_unique": (C.c_int, [_I, _I, C.c_uint64, _P, _P, _P, C.c_size_t, _P]),
     "oea_proje_workspace_bytes": (C.c_size_t, [_I, _I, _I, _I]),
     "oea_proje_score_fed": (C.c_int, [C.POINTER(Proje), _P, _P, _P, _I, _P, _P, _I, _P, C.c_size_t, _P, _P]),
+    "oea_nce_workspace_bytes": (C.c_size_t, [_I, _I, _I, _I]),
+    "oea_nce_score_fed": (C.c_int, [C.POINTER(Nce), _P, _P, _I, _P, _P, _I, C.c_float, _P, C.c_size_t, _P, _P]),
+    "oea_pairs_draw": (C.c_int, [_P, _I, _I, C.c_uint64, _I, _I, _P, _P, _P]),
     "oea_rows_gather_sort": (C.c_int, [_P, _L, _I, _I, _P, _P, _P]),
     "oea_gale_shapley_workspace_bytes": (C.c_size_t, [_I, _I]),
     "oea_gale_shapley": (C.c_int, [_P, _P, _I, _I, _I, _I, _P, _P, C.c_size_t, C.POINTER(C.c_int32), _P]),

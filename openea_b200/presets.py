@@ -177,6 +177,14 @@ def attre(scale="15K"):
                  batch_size=5000 if scale == "15K" else 20000, eval_metric="inner", eval_norm=True, literal_len=5)
 
 
+def attr2vec(scale="15K"):
+    """JAPE's configuration (run/args/jape_args_*.json) with embedding_module = "Attr2Vec": the reference ships no
+    configuration of its own for it."""
+    a = jape(scale)
+    a.embedding_module = "Attr2Vec"
+    return a
+
+
 def jape(scale="15K"):
     """run/args/jape_args_*.json."""
     return _args(embedding_module="JAPE", alignment_module="sharing", dim=100, init="normal", ent_l2_norm=True,
