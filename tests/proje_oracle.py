@@ -69,8 +69,9 @@ def _bn(x, beta):
     return (x - mu) / torch.sqrt(var + BN_EPS) + beta
 
 
-def loss_of(tv, norms, pos, sampled, num_tries):
-    """The batch loss of float64 tensors `tv` (on any device) for host index arrays."""
+def loss_of(tv, norms, pos, sampled, num_tries, drop_true=None):
+    """The batch loss of float64 tensors `tv` (on any device) for host index arrays.  drop_true: a row whose true-class
+    term is left out (tests/nce_edge_cases.py checks that its comparisons can see one term missing)."""
     dev = tv["ent"].device
     h, r, t = (torch.as_tensor(np.asarray(x), dtype=torch.long, device=dev) for x in pos)
     E = l2n(tv["ent"]) if norms["ent"] else tv["ent"]
@@ -85,14 +86,17 @@ def loss_of(tv, norms, pos, sampled, num_tries):
     lq_t, lq_s = lq(pos[2]), lq(sampled)
     true = (X * W[t]).sum(1) + b[t] - lq_t
     samp = X @ W[s].T + b[s] - lq_s
-    return torch.nn.functional.softplus(-true).sum() + torch.nn.functional.softplus(samp).sum()
+    true_terms = torch.nn.functional.softplus(-true)
+    if drop_true is not None:
+        true_terms = torch.cat([true_terms[:drop_true], true_terms[drop_true + 1:]])
+    return true_terms.sum() + torch.nn.functional.softplus(samp).sum()
 
 
-def fwd_bwd(tabs, norms, pos, sampled, num_tries, device="cpu"):
+def fwd_bwd(tabs, norms, pos, sampled, num_tries, device="cpu", drop_true=None):
     """Returns (loss, {name: d loss / d variable as float64 arrays in the shape given}); `device`: where the float64
     graph runs (a 100K-shape batch is a [5 000, 4 096] product)."""
     tv = {k: torch.tensor(np.asarray(v), dtype=torch.float64, device=device, requires_grad=True) for k, v in tabs.items()}
-    val = loss_of(tv, norms, pos, sampled, num_tries)
+    val = loss_of(tv, norms, pos, sampled, num_tries, drop_true)
     val.backward()
     return float(val.detach()), {k: (v.grad.cpu().numpy() if v.grad is not None else np.zeros(v.shape))
                                  for k, v in tv.items()}
