@@ -113,7 +113,7 @@ __device__ __forceinline__ void duo_score_body(const TableDev& ent, const TableD
             const oea_kg_view& kg = P.kg[s.q];
             h = s.h; r = s.r; t = s.t;
             if (P.diag & 1) { neg_e = __ldg(kg.entities + (uint32_t)(p * 31 + hl * 977) % (uint32_t)kg.n_entities); neg_head = (p + hl) & 1; }
-            else sample_negatives<16>(P, seed, kg, live, p, h, r, t, k, lane, ent.w, ent.pitch, neg_e, neg_head);
+            else sample_negatives<16>(P, seed, kg, live, p, h, r, t, k, lane, neg_e, neg_head);
             const unsigned hm_all = __ballot_sync(OEA_FULL, neg_head);
             if (dbg != nullptr && live) dump_draws<16>(dbg, p, k, s, hm_all, lane, neg_e);
         }

@@ -29,7 +29,7 @@ k_sample_batch(SampledParams P, int sampler, const float* __restrict__ warm_w, i
         int neg_e = 0;
         bool neg_head = false;
         if (sampler == 0) {
-            sample_negatives<32>(P, P.seed, kg, true, p, h, r, t, k, lane, warm_w, warm_pitch, neg_e, neg_head);
+            sample_negatives<32>(P, P.seed, kg, true, p, h, r, t, k, lane, neg_e, neg_head);
         } else if (lane < k) {
             const uint32_t base = rng_base(P.seed, (uint32_t)P.step, (uint32_t)p);
             bool done = false;
@@ -56,9 +56,9 @@ k_sample_batch(SampledParams P, int sampler, const float* __restrict__ warm_w, i
                 neg_e = __ldg(kg.entities + bounded32(rng_draw(base, 0xFA11u, (uint32_t)lane), (uint32_t)kg.n_entities));
                 neg_head = false;
             }
-            if (warm_w != nullptr) prefetch_row_l2(warm_w + (size_t)neg_e * warm_pitch, warm_pitch);
         }
         if (lane < k) {
+            if (warm_w != nullptr) prefetch_row_l2(warm_w + (size_t)neg_e * warm_pitch, warm_pitch);   // for the next kernel
             const size_t o = (size_t)p * k + lane;
             neg_out[o] = neg_head ? neg_e : h;
             neg_out[n_neg + o] = r;
@@ -81,7 +81,7 @@ extern "C" int oea_triple_sample_batch(const oea_kg_view* kg1, const oea_kg_view
     if (sampler != 0 && sampler != 1) return OEA_ERR_KIND;
     if (!pos_hrt || !n_pos_host || (smp->neg_per_pos > 0 && !neg_hrt)) return OEA_ERR_NULL;
     if (warm != nullptr) { rc = check_table(warm, false); if (rc) return rc; }
-    if (sampler == 0 && warm == nullptr) return OEA_ERR_NULL;   // the fast sampler prefetches unconditionally
+    if (sampler == 0 && warm == nullptr) return OEA_ERR_NULL;   // the fast sampler always warms the rows it draws
     *n_pos_host = n_pos;
     if (n_pos == 0) return OEA_OK;
     P.diag = 0;

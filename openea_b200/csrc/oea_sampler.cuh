@@ -90,8 +90,7 @@ __device__ __forceinline__ void dump_draws(int32_t* __restrict__ dbg, int p, int
 // the same positive and seed.  A group that is not `live` samples nothing.
 template <int LANES>
 __device__ __forceinline__ void sample_negatives(const SampledParams& P, uint64_t seed, const oea_kg_view& kg, bool live, int p,
-                                                 int h, int r, int t, int k, int lane, const float* __restrict__ ent_w,
-                                                 int ent_pitch, int& neg_e, bool& neg_head) {
+                                                 int h, int r, int t, int k, int lane, int& neg_e, bool& neg_head) {
     static_assert(LANES == 16 || LANES == 32, "a warp or a half-warp");
     const int hl = lane & (LANES - 1);
     const uint32_t group_bit = (uint32_t)(lane / LANES) << 31;   // C <= 2^31: bit 31 separates the half-warps
@@ -126,9 +125,10 @@ __device__ __forceinline__ void sample_negatives(const SampledParams& P, uint64_
             if (__ballot_sync(OEA_FULL, unsettled) == 0u) break;
         }
         if (need) {
+            // No L2 prefetch of the candidate's row here: the scorer's demand loads of it follow within the same
+            // positive, and at the 100K step (memory-system throughput bound, DESIGN.md §4) the extra four line
+            // requests per negative cost more than the latency they hide.
             const int e = __ldg(list + pos);
-            // start fetching the candidate's row while the membership probe is in flight (rejections are < 1 %)
-            prefetch_row_l2(ent_w + (size_t)e * ent_pitch, ent_pitch);
             bool accept = tr == P.max_try - 1;
             if (!accept) {
                 const uint64_t key = head ? triple_key(e, r, t, P.tset.ent_bits, P.tset.rel_bits)

@@ -99,7 +99,7 @@ __device__ __forceinline__ void positive_score_body(const TableDev& ent, const T
             h = s.h; r = s.r; t = s.t;
             // lane j < k owns negative j
             bool neg_head = false;
-            sample_negatives<32>(P, seed, P.kg[s.q], true, p, h, r, t, k, lane, ent.w, ent.pitch, neg_e, neg_head);
+            sample_negatives<32>(P, seed, P.kg[s.q], true, p, h, r, t, k, lane, neg_e, neg_head);
             head_mask = __ballot_sync(OEA_FULL, neg_head);
             if (dbg != nullptr) dump_draws<32>(dbg, p, k, s, head_mask, lane, neg_e);
         }

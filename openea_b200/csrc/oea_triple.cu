@@ -80,7 +80,7 @@ __device__ __forceinline__ void oct_score_body(const TableDev& ent, const TableD
         int neg_e = 0;
         bool neg_head = false;
         if (P.diag & 1) { neg_e = __ldg(kg.entities + (uint32_t)(p * 31 + lane * 977) % (uint32_t)kg.n_entities); neg_head = (p + lane) & 1; }
-        else sample_negatives<32>(P, seed, kg, true, p, h, r, t, k, lane, ent.w, ent.pitch, neg_e, neg_head);
+        else sample_negatives<32>(P, seed, kg, true, p, h, r, t, k, lane, neg_e, neg_head);
         const unsigned head_mask = __ballot_sync(OEA_FULL, neg_head);
         if (dbg != nullptr) dump_draws<32>(dbg, p, k, s, head_mask, lane, neg_e);
 
