@@ -341,6 +341,46 @@ int oea_proje_score_fed(const oea_proje* model, const int32_t* pos_h, const int3
                         int32_t n_pos, const int32_t* sampled, const int32_t* num_tries, int32_t num_sampled,
                         void* workspace, size_t workspace_bytes, double* loss_out, void* stream);
 
+/* ---- path (i), ConvE (models/neural/conve.py) ---------------------------------------------------------------------- */
+
+/* ConvE's variables (conve.py:42-68 on top of ProjE's proje.py:36-44).  ent, rel, cls_w, cls_b as in oea_proje; every
+ * table but cls_b shares pitch <= 128.  With d = dim, (x, y) = dim_factorization(d) (conve.py:10-18) and F = conv->rows:
+ *   conv    [F, 12]: row f holds the 3×3 kernel's taps of filter f (conv2d's [3, 3, 1, F] kernel, tap dy·3 + dx), the
+ *           conv bias, and the gamma and beta of the batch norm over filters (axis = 1)
+ *   bn_in   [2, y]: gamma and beta of the batch norm over the stacked image's columns (axis = −1)
+ *   fc_w    [2·F·d, d]: fully_connected's weights (input index f·2d + i·y + j)
+ *   fc_out  [3, d]: fully_connected's bias, and gamma and beta of the output batch norm
+ * All raw (no l2_normalize); one Adam per table is element-wise, as TF's one optimiser over the separate variables. */
+typedef struct oea_conve {
+    const oea_table* ent;
+    const oea_table* rel;
+    const oea_table* cls_w;
+    const oea_table* cls_b;
+    const oea_table* conv;
+    const oea_table* bn_in;
+    const oea_table* fc_w;
+    const oea_table* fc_out;
+} oea_conve;
+
+/* ConvE's fed step, forward + backward (conve.py:42-79): ê[h] and r̂[r] reshaped row-major to x × y and stacked into a
+ * [2x, y] image; an inference-mode batch norm (moving mean 0, variance 1, ε = 1e-3: v·γ/√(1+ε) + β) per column;
+ * dropout; a 3×3 'same' cross-correlation with F filters and a bias; a batch norm per filter; ReLU; dropout; the
+ * flattened [2Fd] vector through fully_connected (ReLU); a batch norm per column → X; then tf.nn.nce_loss over the given
+ * sampled set exactly as oea_proje_score_fed scores X.  Dropout keeps element i of mask s (0: the image, 1: the conv
+ * output) iff (pcg32(k_s ^ i) >> 8)·2⁻²⁴ < keep_prob with k_s = pcg32(lo(seed) ^ pcg32(hi(seed) + s·0x9E3779B9)), and
+ * scales kept elements by 1/keep_prob; keep_prob = 1 is the identity.  *loss_out (device fp64) += the batch loss; every
+ * table's grad += d loss / d raw variable, touched rows flagged (all rows of conv, bn_in, fc_w, fc_out).  FP32
+ * throughout.  OEA_ERR_RANGE unless 0 < keep_prob <= 1 and 1 <= num_sampled <= cls_w->rows; OEA_ERR_DIM when F < 1,
+ * a pitch exceeds 128 or the pitches or dims disagree; OEA_ERR_SHAPE when a tower table is not of the shape above or
+ * cls_b is not [cls_w->rows, 1]; OEA_ERR_WORKSPACE when the 16-byte aligned workspace is smaller than
+ * oea_conve_workspace_bytes(n_pos, num_sampled, dim, F, cls_w->rows), which also covers oea_logu_sample_unique over
+ * cls_w->rows classes.  Run oea_rowopt_apply on the eight tables afterwards. */
+size_t oea_conve_workspace_bytes(int32_t n_pos, int32_t num_sampled, int32_t dim, int32_t filters, int32_t n_classes);
+int oea_conve_score_fed(const oea_conve* model, const int32_t* pos_h, const int32_t* pos_r, const int32_t* pos_t,
+                        int32_t n_pos, const int32_t* sampled, const int32_t* num_tries, int32_t num_sampled,
+                        float keep_prob, uint64_t dropout_seed, void* workspace, size_t workspace_bytes,
+                        double* loss_out, void* stream);
+
 /* ---- path (i), the general sampled-NCE step (approaches/attr2vec.py) ---------------------------------------------- */
 
 /* The variables of tf.nn.nce_loss applied to an embedding lookup.  in and cls_w share dim and a pitch <= 128; each is

@@ -48,6 +48,17 @@
 //                           class can also be a label; the Jacobian is linear, so the two parts are pushed separately)
 //   6. k_nce_in_push        one warp per row: dX through the input table's normalisation into its gradient
 //
+// oea_conve_score_fed (models/neural/conve.py:42-79): two memsets and thirteen kernels, ProjE's head among them unchanged:
+//   1. k_conve_conv_fwd     one CTA per positive: the stacked image, its batch norm and dropout (kept in img), the 3×3
+//                           convolution, the per-filter batch norm, ReLU and dropout → A [n, 2Fd]
+//   2. k_conve_fc_fwd       Z = A·W on the head's register tile, split over the 2Fd inputs; k_conve_fc_out: bias, ReLU and
+//                           the output batch norm → X
+//   3. the head: k_nce_logq, k_nce_logits / k_nce_dx / k_nce_dw <GatheredW>, k_proje_true
+//   4. k_conve_fc_out_bwd   dX → dz; k_conve_fc_dw: dW = Aᵀ·dz; k_conve_fc_dx: dA = dz·Wᵀ through the ReLU and dropout,
+//                           written over A
+//   5. k_conve_conv_dw      the convolution's and its batch norm's gradients per filter; k_conve_conv_dx: one CTA per
+//                           positive back to the image, through its dropout and batch norm, and into ent.grad, rel.grad
+//
 // oea_pairs_draw: B distinct rows of an [n, 2] pair array, row i = feistel_perm(i, n, key(seed, epoch, step)) for i < B.
 #include "oea_rowmath.cuh"
 
@@ -713,6 +724,372 @@ static HeadGrids head_grids(int n, int S, int ldg) {
     return h;
 }
 
+// ---- ConvE's tower (oea_conve_score_fed) ----------------------------------------------------------------------------
+// An inference-mode batch norm at its initial moving moments (mean 0, variance 1) scales by γ/√(1 + ε) and shifts by β.
+constexpr float kBnInfer = 0.99950037468777f;     // 1/√(1 + 1e-3)
+constexpr int kConvCols = 12;                      // conv table row f: 9 taps (dy·3 + dx), bias, γ₂, β₂
+
+struct ConveDev {
+    TableDev conv, bn_in, fc_w, fc_out;            // [F, 12]; [2, y] γ₁, β₁; [2Fd, d]; [3, d] bias, γ₃, β₃
+    int x, y, F, K, lda;                           // image rows per vector, columns; filters; 2Fd and A's row stride
+    float keep;
+    uint64_t seed;
+};
+
+// tf.nn.dropout's mask as a pure function of (seed, site, flat index): element i of site s is kept iff
+// u = (pcg32(key_s ^ i) >> 8)·2⁻²⁴ < keep, key_s = pcg32(lo(seed) ^ pcg32(hi(seed) + s·0x9E3779B9)).  keep = 1 keeps all.
+__host__ __device__ __forceinline__ uint32_t dropout_key(uint64_t seed, uint32_t site) {
+    return pcg32((uint32_t)seed ^ pcg32((uint32_t)(seed >> 32) + site * 0x9E3779B9u));
+}
+__host__ __device__ __forceinline__ bool dropout_kept(uint32_t key, uint32_t i, float keep) {
+    return (float)(pcg32(key ^ i) >> 8) * 0x1.0p-24f < keep;
+}
+
+// one CTA per positive: ê[h], r̂[r] stacked into the [2x, y] image, the input BN (per column) and dropout into img
+// [n, 2d]; the 3×3 'same' cross-correlation, the per-filter BN, ReLU and dropout into A [n, lda] (index f·2d + i·y + j)
+__global__ void __launch_bounds__(kThreads)
+k_conve_conv_fwd(ProjeDev T, ConveDev C, const int32_t* __restrict__ ph, const int32_t* __restrict__ pr, int n,
+                 float* __restrict__ img, float* __restrict__ A) {
+    __shared__ __align__(16) float s_raw[2][kProjeMaxPitch];
+    __shared__ float s_img[2 * kProjeMaxPitch];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int d = T.dim, D2 = 2 * d, y = C.y, H = 2 * C.x;
+    const uint32_t key0 = dropout_key(C.seed, 0), key1 = dropout_key(C.seed, 1);
+    for (int b = blockIdx.x; b < n; b += gridDim.x) {
+        if (warp < 2) {
+            const Row<1> v = lookup<1>(pick_table(warp == 0, T.ent, T.rel), __ldg((warp == 0 ? ph : pr) + b), lane).x;
+            if (4 * lane < T.pitch) *reinterpret_cast<float4*>(&s_raw[warp][4 * lane]) = v.v[0];
+        }
+        __syncthreads();
+        for (int e = threadIdx.x; e < D2; e += blockDim.x) {
+            const int j = e % y, half = e >= d;
+            const float u = fmaf(s_raw[half][e - half * d], C.bn_in.w[j] * kBnInfer, C.bn_in.w[C.bn_in.pitch + j]);
+            const float v = dropout_kept(key0, (uint32_t)(b * D2 + e), C.keep) ? u / C.keep : 0.f;
+            s_img[e] = v;
+            img[(size_t)b * D2 + e] = v;
+        }
+        __syncthreads();
+        for (int o = threadIdx.x; o < C.lda; o += blockDim.x) {
+            float v = 0.f;
+            if (o < C.K) {
+                const int f = o / D2, pos = o - f * D2, i = pos / y, j = pos - i * y;
+                const float* k = C.conv.w + (size_t)f * C.conv.pitch;
+                float q = k[9];
+#pragma unroll
+                for (int dy = 0; dy < 3; ++dy) {
+                    const int ii = i + dy - 1;
+                    if (ii < 0 || ii >= H) continue;
+#pragma unroll
+                    for (int dx = 0; dx < 3; ++dx) {
+                        const int jj = j + dx - 1;
+                        if (jj >= 0 && jj < y) q = fmaf(k[3 * dy + dx], s_img[ii * y + jj], q);
+                    }
+                }
+                const float p = fmaf(q, k[10] * kBnInfer, k[11]);
+                if (p > 0.f && dropout_kept(key1, (uint32_t)b * (uint32_t)C.K + (uint32_t)o, C.keep)) v = p / C.keep;
+            }
+            A[(size_t)b * C.lda + o] = v;                 // columns K … lda − 1 stay zero for the GEMMs' float4 loads
+        }
+        __syncthreads();
+    }
+}
+
+// Z[b][:] += Σ_{k in split} A[b][k]·W[k][:] over tile t = (batch tile, split of the lda inputs); Z was zeroed
+__global__ void __launch_bounds__(kThreads)
+k_conve_fc_fwd(ProjeDev T, ConveDev C, int n, const float* __restrict__ A, int split, float* __restrict__ z) {
+    __shared__ __align__(16) float As[kTk * kTld];
+    __shared__ __align__(16) float Bs[kTk * kTld];
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    const int mt = (n + kTile - 1) / kTile, st = (C.lda + split - 1) / split;
+    for (int t = blockIdx.x; t < mt * st; t += gridDim.x) {
+        const int m0 = (t % mt) * kTile, k0s = (t / mt) * split, k1s = min(C.lda, k0s + split), kw = min(k1s, C.K);
+        float acc[8][8];
+        zero_acc(acc);
+        for (int k0 = k0s; k0 < k1s; k0 += kTk) {
+            __syncthreads();
+            stage_rows_t(As, [&](int i) { return m0 + i < n ? A + (size_t)(m0 + i) * C.lda : nullptr; }, k0, k1s);
+            stage_rows_n(Bs, [&](int k) { return k0 + k < kw ? C.fc_w.w + (size_t)(k0 + k) * T.pitch : nullptr; }, T.pitch);
+            __syncthreads();
+            tile_mma(acc, As, Bs, ty, tx);
+        }
+#pragma unroll
+        for (int a = 0; a < 8; ++a) {
+            const int m = m0 + ty + 16 * a;
+            if (m >= n) continue;
+#pragma unroll
+            for (int b = 0; b < 8; ++b) {
+                const int c = tx + 16 * b;
+                if (c < T.dim) atomicAdd(z + (size_t)m * T.pitch + c, acc[a][b]);
+            }
+        }
+    }
+}
+
+// the dense layer's bias and ReLU and the output BN: z += bias (kept for the backward), X = γ₃·relu(z)/√(1+ε) + β₃
+__global__ void __launch_bounds__(kThreads)
+k_conve_fc_out(ProjeDev T, ConveDev C, int n, float* __restrict__ z, float* __restrict__ x) {
+    const int P = T.pitch;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < (size_t)n * P; i += (size_t)gridDim.x * blockDim.x) {
+        const int c = (int)(i % P);
+        if (c >= T.dim) { x[i] = 0.f; continue; }           // padding columns of X stay zero for the head's float4 loads
+        const float v = z[i] + C.fc_out.w[c];
+        z[i] = v;
+        x[i] = fmaf(v > 0.f ? v : 0.f, C.fc_out.w[P + c] * kBnInfer, C.fc_out.w[2 * P + c]);
+    }
+}
+
+// back through the output BN and the dense ReLU: dX → dz in place; the column sums are the gradients of the dense bias,
+// γ₃ and β₃.  Thread column c = threadIdx.x % 128, two rows per block step.  Flags every row of the tower's tables.
+__global__ void __launch_bounds__(kThreads)
+k_conve_fc_out_bwd(ProjeDev T, ConveDev C, int n, const float* __restrict__ z, float* __restrict__ dx) {
+    __shared__ float s_sum[3][kThreads];
+    const int P = T.pitch, c = threadIdx.x & (kProjeMaxPitch - 1), r0 = threadIdx.x / kProjeMaxPitch;
+    float sb = 0.f, sg = 0.f, sbeta = 0.f;
+    if (c < P) {
+        const float g3 = c < T.dim ? C.fc_out.w[P + c] * kBnInfer : 0.f;
+        for (int b = 2 * blockIdx.x + r0; b < n; b += 2 * gridDim.x) {
+            const size_t i = (size_t)b * P + c;
+            const float g = dx[i], v = z[i];
+            const float dz = v > 0.f ? g * g3 : 0.f;
+            dx[i] = dz;
+            sb += dz;
+            sg = fmaf(g, (v > 0.f ? v : 0.f) * kBnInfer, sg);
+            sbeta += g;
+        }
+    }
+    s_sum[0][threadIdx.x] = sb; s_sum[1][threadIdx.x] = sg; s_sum[2][threadIdx.x] = sbeta;
+    __syncthreads();
+    if (threadIdx.x < kProjeMaxPitch && c < T.dim)
+        for (int r = 0; r < 3; ++r)
+            atomicAdd(C.fc_out.g + (size_t)r * P + c, s_sum[r][c] + s_sum[r][c + kProjeMaxPitch]);
+    const int gt = blockIdx.x * blockDim.x + threadIdx.x, gs = gridDim.x * blockDim.x;
+    for (int r = gt; r < C.K; r += gs) C.fc_w.touched[r] = 1;
+    for (int r = gt; r < C.F; r += gs) C.conv.touched[r] = 1;
+    if (gt < 2) C.bn_in.touched[gt] = 1;
+    if (gt < 3) C.fc_out.touched[gt] = 1;
+}
+
+// dW[k][:] += Σ_{b in split} A[b][k]·dz[b][:] over tile t = (input tile, split of the batch)
+__global__ void __launch_bounds__(kThreads)
+k_conve_fc_dw(ProjeDev T, ConveDev C, int n, const float* __restrict__ A, const float* __restrict__ dz, int split) {
+    __shared__ __align__(16) float As[kTk * kTld];
+    __shared__ __align__(16) float Bs[kTk * kTld];
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    const int mt = (C.K + kTile - 1) / kTile, bt = (n + split - 1) / split;
+    for (int t = blockIdx.x; t < mt * bt; t += gridDim.x) {
+        const int m0 = (t % mt) * kTile, b0 = (t / mt) * split, b1 = min(n, b0 + split);
+        float acc[8][8];
+        zero_acc(acc);
+        for (int k0 = b0; k0 < b1; k0 += kTk) {
+            __syncthreads();
+            // A's rows run along k, so the slice is staged without a transpose
+            stage_rows_n(As, [&](int k) { return k0 + k < b1 ? A + (size_t)(k0 + k) * C.lda + m0 : nullptr; },
+                         min(kTile, C.lda - m0));
+            stage_rows_n(Bs, [&](int k) { return k0 + k < b1 ? dz + (size_t)(k0 + k) * T.pitch : nullptr; }, T.pitch);
+            __syncthreads();
+            tile_mma(acc, As, Bs, ty, tx);
+        }
+        __syncthreads();
+        float* Cs = As;                                   // 16 rows at a time, as k_nce_dw
+#pragma unroll
+        for (int a = 0; a < 8; ++a) {
+#pragma unroll
+            for (int b = 0; b < 8; ++b) Cs[ty * kTld + tx + 16 * b] = acc[a][b];
+            __syncthreads();
+            for (int e = threadIdx.x; e < 16 * (kTile / 4); e += blockDim.x) {
+                const int r = e >> 5, c = 4 * (e & 31), k = m0 + r + 16 * a;
+                if (k < C.K && c < T.pitch)
+                    red_add4(C.fc_w.g + (size_t)k * T.pitch + c, *reinterpret_cast<const float4*>(Cs + r * kTld + c));
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// dA = dz·Wᵀ, taken back through the conv ReLU and dropout in the epilogue and written over A: the ReLU was active and
+// the element kept iff A > 0, where dp = dA/keep.  Tile t = (batch tile, input tile).
+__global__ void __launch_bounds__(kThreads)
+k_conve_fc_dx(ProjeDev T, ConveDev C, int n, const float* __restrict__ dz, float* A) {
+    __shared__ __align__(16) float As[kTk * kTld];
+    __shared__ __align__(16) float Bs[kTk * kTld];
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    const int mt = (n + kTile - 1) / kTile, nt = (C.lda + kTile - 1) / kTile;
+    for (int t = blockIdx.x; t < mt * nt; t += gridDim.x) {
+        const int m0 = (t % mt) * kTile, n0 = (t / mt) * kTile;
+        float acc[8][8];
+        zero_acc(acc);
+        for (int k0 = 0; k0 < T.pitch; k0 += kTk) {
+            __syncthreads();
+            stage_rows_t(As, [&](int i) { return m0 + i < n ? dz + (size_t)(m0 + i) * T.pitch : nullptr; }, k0, T.pitch);
+            stage_rows_t(Bs, [&](int i) { return n0 + i < C.K ? C.fc_w.w + (size_t)(n0 + i) * T.pitch : nullptr; }, k0,
+                         T.pitch);
+            __syncthreads();
+            tile_mma(acc, As, Bs, ty, tx);
+        }
+#pragma unroll
+        for (int a = 0; a < 8; ++a) {
+            const int m = m0 + ty + 16 * a;
+            if (m >= n) continue;
+#pragma unroll
+            for (int b = 0; b < 8; ++b) {
+                const int k = n0 + tx + 16 * b;
+                if (k >= C.lda) continue;
+                float* p = A + (size_t)m * C.lda + k;
+                *p = *p > 0.f ? acc[a][b] / C.keep : 0.f;
+            }
+        }
+    }
+}
+
+// the gradients of filter f's taps, bias, γ₂ and β₂ over one split of the batch: tile t = (filter, batch split).
+// The conv output q is recomputed from img (nine FMAs) rather than stored: it is needed only for γ₂.
+__global__ void __launch_bounds__(kThreads)
+k_conve_conv_dw(ProjeDev T, ConveDev C, int n, const float* __restrict__ img, const float* __restrict__ dp, int split) {
+    __shared__ float s_red[kWarpsPerBlock][kConvCols];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int D2 = 2 * T.dim, y = C.y, H = 2 * C.x;
+    const int bt = (n + split - 1) / split;
+    for (int t = blockIdx.x; t < C.F * bt; t += gridDim.x) {
+        const int f = t % C.F, b0 = (t / C.F) * split, b1 = min(n, b0 + split);
+        const float* k = C.conv.w + (size_t)f * C.conv.pitch;
+        const float s2 = k[10] * kBnInfer;
+        float acc[kConvCols];
+#pragma unroll
+        for (int r = 0; r < kConvCols; ++r) acc[r] = 0.f;
+        for (int e = threadIdx.x; e < (b1 - b0) * D2; e += blockDim.x) {
+            const int b = b0 + e / D2, pos = e % D2, i = pos / y, j = pos - i * y;
+            const float g = dp[(size_t)b * C.lda + f * D2 + pos];
+            if (g == 0.f) continue;                       // dropped or ReLU inactive: no contribution
+            const float* im = img + (size_t)b * D2;
+            float nb[9];
+            float q = k[9];
+#pragma unroll
+            for (int dy = 0; dy < 3; ++dy)
+#pragma unroll
+                for (int dx = 0; dx < 3; ++dx) {
+                    const int ii = i + dy - 1, jj = j + dx - 1;
+                    nb[3 * dy + dx] = (ii >= 0 && ii < H && jj >= 0 && jj < y) ? im[ii * y + jj] : 0.f;
+                    q = fmaf(k[3 * dy + dx], nb[3 * dy + dx], q);
+                }
+            const float dq = g * s2;
+#pragma unroll
+            for (int r = 0; r < 9; ++r) acc[r] = fmaf(dq, nb[r], acc[r]);
+            acc[9] += dq;
+            acc[10] = fmaf(g, q * kBnInfer, acc[10]);
+            acc[11] += g;
+        }
+#pragma unroll
+        for (int r = 0; r < kConvCols; ++r) {
+            const float v = warp_sum(acc[r]);
+            if (lane == 0) s_red[warp][r] = v;
+        }
+        __syncthreads();
+        if (threadIdx.x < kConvCols) {
+            float s = 0.f;
+            for (int w = 0; w < kWarpsPerBlock; ++w) s += s_red[w][threadIdx.x];
+            atomicAdd(C.conv.g + (size_t)f * C.conv.pitch + threadIdx.x, s);
+        }
+        __syncthreads();
+    }
+}
+
+// one CTA per positive: the transposed convolution of dq = dp·γ₂/√(1+ε) back to the image, through the dropout and the
+// input BN (γ₁, β₁ column sums), and dê, dr̂ through the tables' normalisation into ent.grad, rel.grad
+__global__ void __launch_bounds__(kThreads)
+k_conve_conv_dx(ProjeDev T, ConveDev C, const int32_t* __restrict__ ph, const int32_t* __restrict__ pr, int n,
+                const float* __restrict__ dp) {
+    __shared__ __align__(16) float s_v[2][kProjeMaxPitch];
+    __shared__ __align__(16) float s_dv[2][kProjeMaxPitch];
+    __shared__ float s_g1[kProjeMaxPitch], s_b1[kProjeMaxPitch];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int d = T.dim, D2 = 2 * d, y = C.y, H = 2 * C.x;
+    const uint32_t key0 = dropout_key(C.seed, 0);
+    for (int i = threadIdx.x; i < kProjeMaxPitch; i += blockDim.x) {
+        s_g1[i] = s_b1[i] = 0.f;
+        s_dv[0][i] = s_dv[1][i] = 0.f;                    // columns d … pitch − 1 are pushed as zeros
+    }
+    for (int b = blockIdx.x; b < n; b += gridDim.x) {
+        NRow<1> nr;
+        int id = 0;
+        if (warp < 2) {
+            id = __ldg((warp == 0 ? ph : pr) + b);
+            nr = lookup<1>(pick_table(warp == 0, T.ent, T.rel), id, lane);
+            if (4 * lane < T.pitch) *reinterpret_cast<float4*>(&s_v[warp][4 * lane]) = nr.x.v[0];
+        }
+        __syncthreads();
+        const float* g = dp + (size_t)b * C.lda;
+        for (int e = threadIdx.x; e < D2; e += blockDim.x) {
+            const int i = e / y, j = e - i * y, half = e >= d;
+            float du = 0.f;
+            for (int f = 0; f < C.F; ++f) {
+                const float* k = C.conv.w + (size_t)f * C.conv.pitch;
+                const float* gf = g + f * D2;
+                float s = 0.f;
+#pragma unroll
+                for (int dy = 0; dy < 3; ++dy) {
+                    const int ii = i - dy + 1;                // the output row whose tap dy reads image row i
+                    if (ii < 0 || ii >= H) continue;
+#pragma unroll
+                    for (int dx = 0; dx < 3; ++dx) {
+                        const int jj = j - dx + 1;
+                        if (jj >= 0 && jj < y) s = fmaf(k[3 * dy + dx], __ldg(gf + ii * y + jj), s);
+                    }
+                }
+                du = fmaf(s, k[10] * kBnInfer, du);
+            }
+            du = dropout_kept(key0, (uint32_t)(b * D2 + e), C.keep) ? du / C.keep : 0.f;
+            atomicAdd(s_g1 + j, du * s_v[half][e - half * d] * kBnInfer);
+            atomicAdd(s_b1 + j, du);
+            s_dv[half][e - half * d] = du * C.bn_in.w[j] * kBnInfer;
+        }
+        __syncthreads();
+        if (warp < 2) {
+            Row<1> gr;
+            gr.v[0] = 4 * lane < kProjeMaxPitch ? *reinterpret_cast<const float4*>(&s_dv[warp][4 * lane]) : f4(0.f);
+            push<1>(pick_table(warp == 0, T.ent, T.rel), id, lane, gr, nr);
+        }
+        __syncthreads();
+    }
+    for (int j = threadIdx.x; j < y; j += blockDim.x) {
+        atomicAdd(C.bn_in.g + j, s_g1[j]);
+        atomicAdd(C.bn_in.g + C.bn_in.pitch + j, s_b1[j]);
+    }
+}
+
+// dim_factorization of models/neural/conve.py:10-18: x = the largest divisor of d not above ⌊√d⌋ + 1, y = d / x
+static void conve_factor(int d, int* x, int* y) {
+    int half = (int)sqrt((double)d) + 1;
+    while (d % half > 0) --half;
+    *x = half;
+    *y = d / half;
+}
+
+struct ConveWs {
+    size_t first, img, a, z, x, dx, lq, g, total;
+    int ldg, lda;
+};
+
+// workspace sections, each 256-B aligned: the sampler's first-draw index per class, the dropped image [n, 2d], the dense
+// layer's input A [n, lda] (its gradient dp overwrites it in the backward), z, X and dX [n, pitch], log q [S], G [n, ldg]
+static ConveWs conve_layout(int n, int num_sampled, int dim, int pitch, int filters, int n_classes) {
+    ConveWs w;
+    size_t at = 0;
+    auto take = [&](size_t bytes) { const size_t o = at; at += (bytes + 255) & ~(size_t)255; return o; };
+    const size_t row = 4 * (size_t)n * pitch;
+    w.ldg = (num_sampled + 3) / 4 * 4;
+    w.lda = (2 * filters * dim + 3) / 4 * 4;
+    w.first = take(4 * (size_t)n_classes);
+    w.img = take(4 * (size_t)n * 2 * dim);
+    w.a = take(4 * (size_t)n * w.lda);
+    w.z = take(row);
+    w.x = take(row);
+    w.dx = take(row);
+    w.lq = take(4 * (size_t)num_sampled);
+    w.g = take(4 * (size_t)n * w.ldg);
+    w.total = at;
+    return w;
+}
+
 }  // namespace oea
 
 using namespace oea;
@@ -862,6 +1239,101 @@ extern "C" int oea_pairs_draw(const int32_t* pairs, int32_t n_pairs, int32_t bat
     if (pairs == nullptr || first == nullptr || second == nullptr) return OEA_ERR_NULL;
     OEA_LAUNCH_STRIDED(k_pairs_draw, (batch + kThreads - 1) / kThreads, kThreads, 0, (cudaStream_t)stream, pairs,
                        (uint32_t)n_pairs, batch, pairs_key(seed, epoch, step), first, second);
+    OEA_LAUNCH_CHECK();
+    return OEA_OK;
+}
+
+extern "C" size_t oea_conve_workspace_bytes(int32_t n_pos, int32_t num_sampled, int32_t dim, int32_t filters,
+                                            int32_t n_classes) {
+    if (n_pos < 0 || num_sampled < 1 || dim <= 0 || filters < 1 || n_classes <= 0) return 0;
+    return conve_layout(n_pos, num_sampled, dim, (dim + 3) / 4 * 4, filters, n_classes).total;
+}
+
+extern "C" int oea_conve_score_fed(const oea_conve* model, const int32_t* pos_h, const int32_t* pos_r,
+                                   const int32_t* pos_t, int32_t n_pos, const int32_t* sampled, const int32_t* num_tries,
+                                   int32_t num_sampled, float keep_prob, uint64_t dropout_seed, void* workspace,
+                                   size_t workspace_bytes, double* loss_out, void* stream) {
+    if (model == nullptr) return OEA_ERR_NULL;
+    const oea_table* tabs[8] = {model->ent, model->rel, model->cls_w, model->cls_b, model->conv, model->bn_in,
+                                model->fc_w, model->fc_out};
+    for (const oea_table* t : tabs) {
+        const int rc = check_table(t, true);
+        if (rc) return rc;
+    }
+    const oea_table *ent = model->ent, *rel = model->rel, *w = model->cls_w, *b = model->cls_b;
+    const oea_table *conv = model->conv, *bn_in = model->bn_in, *fc_w = model->fc_w, *fc_out = model->fc_out;
+    const int d = ent->dim, P = ent->pitch, F = conv->rows;
+    if (rel->dim != d || w->dim != d || rel->pitch != P || w->pitch != P || fc_w->pitch != P || fc_out->pitch != P ||
+        P > kProjeMaxPitch)
+        return OEA_ERR_DIM;
+    if (F < 1) return OEA_ERR_DIM;
+    int fx, fy;
+    conve_factor(d, &fx, &fy);
+    if (b->rows != w->rows || b->dim != 1 || conv->dim != kConvCols || bn_in->rows != 2 || bn_in->dim != fy ||
+        fc_w->rows != 2 * F * d || fc_w->dim != d || fc_out->rows != 3 || fc_out->dim != d)
+        return OEA_ERR_SHAPE;
+    if (!(keep_prob > 0.f && keep_prob <= 1.f)) return OEA_ERR_RANGE;
+    if (num_sampled < 1 || num_sampled > w->rows) return OEA_ERR_RANGE;
+    if (n_pos < 0) return OEA_ERR_SHAPE;
+    if (sampled == nullptr || num_tries == nullptr || loss_out == nullptr) return OEA_ERR_NULL;
+    if (n_pos > 0 && (!pos_h || !pos_r || !pos_t)) return OEA_ERR_NULL;
+    const ConveWs L = conve_layout(n_pos, num_sampled, d, P, F, w->rows);
+    if (workspace == nullptr || workspace_bytes < L.total || !aligned16(workspace)) return OEA_ERR_WORKSPACE;
+    if (n_pos == 0) return OEA_OK;
+
+    char* ws = static_cast<char*>(workspace);
+    float* img = reinterpret_cast<float*>(ws + L.img);
+    float* A = reinterpret_cast<float*>(ws + L.a);
+    float* z = reinterpret_cast<float*>(ws + L.z);
+    float* x = reinterpret_cast<float*>(ws + L.x);
+    float* dx = reinterpret_cast<float*>(ws + L.dx);
+    float* lq = reinterpret_cast<float*>(ws + L.lq);
+    float* G = reinterpret_cast<float*>(ws + L.g);
+    ProjeDev T{};
+    T.ent = table_dev(ent); T.rel = table_dev(rel); T.w = table_dev(w); T.b = table_dev(b);
+    T.w.norm = T.b.norm = false;                          // entity_w and entity_b: raw
+    T.dim = d; T.pitch = P; T.n_classes = w->rows; T.num_sampled = num_sampled; T.ldg = L.ldg;
+    ConveDev C;
+    C.conv = table_dev(conv); C.bn_in = table_dev(bn_in); C.fc_w = table_dev(fc_w); C.fc_out = table_dev(fc_out);
+    C.x = fx; C.y = fy; C.F = F; C.K = 2 * F * d; C.lda = L.lda; C.keep = keep_prob; C.seed = dropout_seed;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int n = n_pos, S = num_sampled;
+    const HeadGrids H = head_grids(n, S, L.ldg);
+#ifdef OEA_HOST_EMU
+    const int pos_grid = 2, fwd_grid = 2, dw_grid = 2, dx_grid = 2, conv_grid = 2, out_grid = 2, bwd_grid = 2;
+    const int split_k = 2 * kTk, split_b = 2 * kTk, split_conv = 7;
+#else
+    // split the dense layer's reductions so that about two CTAs per SM run (a batch of 500 is four row tiles; d = 100
+    // is one column tile), and the per-filter sums of the conv backward over about two CTAs per SM as well
+    const int sms = sm_count_cached(), want = 2 * sms;
+    const int mt_b = (n + kTile - 1) / kTile, mt_k = (C.K + kTile - 1) / kTile;
+    auto split_of = [](int len, int parts) { const int s = (len + parts - 1) / parts; return (s + kTk - 1) / kTk * kTk; };
+    const int split_k = split_of(L.lda, (want + mt_b - 1) / mt_b);
+    const int split_b = split_of(n, (want + mt_k - 1) / mt_k);
+    const int conv_parts = (want + F - 1) / F, split_conv = (n + conv_parts - 1) / conv_parts;
+    const int pos_grid = min(n, 8 * sms);
+    const int fwd_grid = mt_b * ((L.lda + split_k - 1) / split_k);
+    const int dw_grid = mt_k * ((n + split_b - 1) / split_b);
+    const int dx_grid = mt_b * ((L.lda + kTile - 1) / kTile);
+    const int conv_grid = F * ((n + split_conv - 1) / split_conv);
+    const int out_grid = min((int)(((size_t)n * P + kThreads - 1) / kThreads), 8 * sms);
+    const int bwd_grid = min((n + 1) / 2, sms);           // two rows per block step; one flush of 3·d sums per block
+#endif
+    OEA_CUDA_TRY(cudaMemsetAsync(z, 0, 4 * (size_t)n * P, st));
+    OEA_CUDA_TRY(cudaMemsetAsync(dx, 0, 4 * (size_t)n * P, st));
+    OEA_LAUNCH(k_conve_conv_fwd, pos_grid, kThreads, 0, st, T, C, pos_h, pos_r, n, img, A);
+    OEA_LAUNCH(k_conve_fc_fwd, fwd_grid, kThreads, 0, st, T, C, n, A, split_k, z);
+    OEA_LAUNCH(k_conve_fc_out, out_grid, kThreads, 0, st, T, C, n, z, x);
+    OEA_LAUNCH(k_nce_logq, H.rows, kThreads, 0, st, sampled, num_tries, T.n_classes, S, lq);
+    OEA_LAUNCH(k_nce_logits<GatheredW>, H.lg, kThreads, 0, st, T, n, x, sampled, lq, G, loss_out, GatheredW{});
+    OEA_LAUNCH(k_nce_dx<GatheredW>, H.dx, kThreads, 0, st, T, n, G, sampled, H.split_s, dx, GatheredW{});
+    OEA_LAUNCH(k_nce_dw<GatheredW>, H.dw, kThreads, 0, st, T, n, G, x, sampled, H.split_b, GatheredW{});
+    OEA_LAUNCH(k_proje_true, H.rows, kThreads, 0, st, T, pos_t, n, x, num_tries, dx, loss_out);
+    OEA_LAUNCH(k_conve_fc_out_bwd, bwd_grid, kThreads, 0, st, T, C, n, z, dx);
+    OEA_LAUNCH(k_conve_fc_dw, dw_grid, kThreads, 0, st, T, C, n, A, dx, split_b);
+    OEA_LAUNCH(k_conve_fc_dx, dx_grid, kThreads, 0, st, T, C, n, dx, A);
+    OEA_LAUNCH(k_conve_conv_dw, conv_grid, kThreads, 0, st, T, C, n, img, A, split_conv);
+    OEA_LAUNCH(k_conve_conv_dx, pos_grid, kThreads, 0, st, T, C, pos_h, pos_r, n, A);
     OEA_LAUNCH_CHECK();
     return OEA_OK;
 }

@@ -616,6 +616,53 @@ class ProjETrainer:
         return v
 
 
+class ConvETrainer(ProjETrainer):
+    """ConvE's step (models/neural/conve.py:42-79): ProjE's batch producer, sampler, Adam and loss accumulator, with the
+    convolution tower in front of the NCE head (oea_conve_score_fed).  tables = (ent, rel, cls_w, cls_b, conv, bn_in,
+    fc_w, fc_out) EmbeddingTables (include/oea.h oea_conve).  The dropout masks are keyed by a seed derived from the
+    sampler's, so a step's masks, like its sampled set, are a function of (epoch seed, step) only."""
+
+    def __init__(self, tables, num_sampled, lr, keep_prob, sampler="fast"):
+        super().__init__(tables, num_sampled, lr, sampler)
+        self.keep_prob = float(keep_prob)
+        if not 0.0 < self.keep_prob <= 1.0:
+            raise ValueError("output_keep_prob = %r is not in (0, 1]" % keep_prob)
+        self.filters = self.tables[4].rows
+
+    def _workspace(self, n_pos):
+        need = self.lib.oea_conve_workspace_bytes(n_pos, self.num_sampled, self.tables[0].dim, self.filters,
+                                                  self.tables[2].rows)
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(max(1, need), dtype=torch.uint8, device=self.tables[0].device)
+        return self._ws
+
+    def score_fed(self, pos, sampled=None, num_tries=None, dropout_seed=0, loss_out=None):
+        """pos: int32 device tensor [3, n] (h | r | t rows); sampled / num_tries: int32 device tensors (default: the
+        last sample()).  Accumulates gradients into the eight tables and adds the batch loss into loss_out."""
+        out = self.loss_dev if loss_out is None else loss_out
+        sampled = self.sampled if sampled is None else sampled
+        num_tries = self.num_tries if num_tries is None else num_tries
+        n_pos = pos.shape[1]
+        ws = self._workspace(n_pos)
+        model = L.Conve(*[C.pointer(t.c_struct()) for t in self.tables])
+        np_ = lambda i: C.c_void_p(0 if n_pos == 0 else pos[i].data_ptr())
+        L.check(self.lib.oea_conve_score_fed(C.byref(model), np_(0), np_(1), np_(2), n_pos, _ptr(sampled),
+                                             _ptr(num_tries), sampled.numel(), self.keep_prob,
+                                             int(dropout_seed) & (2**64 - 1), _ptr(ws), ws.numel(), _ptr(out),
+                                             _stream_ptr()), "oea_conve_score_fed")
+
+    def step_sampled(self, kg1, kg2, tset, batch_size, neg_per_pos, step, epoch_seed, max_try=10, **_):
+        """One session.run([triple_loss, triple_optimizer]) of conve.py:42-79; neg_per_pos is ignored (positives only)."""
+        pos = self.sample_batch(kg1, kg2, tset, batch_size, step, epoch_seed, max_try)
+        if pos.shape[1] == 0:
+            return 0
+        seed = self.step_seed(epoch_seed, step)
+        self.sample(seed)
+        self.score_fed(pos, dropout_seed=self.step_seed(seed, 0))
+        self.apply()
+        return pos.shape[1]
+
+
 class NceTrainer:
     """tf.nn.nce_loss applied to an embedding lookup, one reduce_mean step of approaches/attr2vec.py:113-124,145-161:
     B distinct pairs drawn on the device (oea_pairs_draw, keyed by (seed, epoch, step)) → TF's unique log-uniform

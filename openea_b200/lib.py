@@ -92,6 +92,12 @@ class Proje(C.Structure):
     _fields_ = [("ent", _TP), ("rel", _TP), ("cls_w", _TP), ("cls_b", _TP), ("params", _TP)]
 
 
+class Conve(C.Structure):
+    # oea_conve: ProjE's four tables, then the tower's: conv [F, 12], bn_in [2, y], fc_w [2Fd, d], fc_out [3, d]
+    _fields_ = [("ent", _TP), ("rel", _TP), ("cls_w", _TP), ("cls_b", _TP), ("conv", _TP), ("bn_in", _TP),
+                ("fc_w", _TP), ("fc_out", _TP)]
+
+
 class Nce(C.Structure):
     # oea_nce: the input table, the class table and the class biases ([C, 1])
     _fields_ = [("in_", _TP), ("cls_w", _TP), ("cls_b", _TP)]
@@ -163,6 +169,9 @@ SIGNATURES = {
     "oea_logu_sample_unique": (C.c_int, [_I, _I, C.c_uint64, _P, _P, _P, C.c_size_t, _P]),
     "oea_proje_workspace_bytes": (C.c_size_t, [_I, _I, _I, _I]),
     "oea_proje_score_fed": (C.c_int, [C.POINTER(Proje), _P, _P, _P, _I, _P, _P, _I, _P, C.c_size_t, _P, _P]),
+    "oea_conve_workspace_bytes": (C.c_size_t, [_I, _I, _I, _I, _I]),
+    "oea_conve_score_fed": (C.c_int, [C.POINTER(Conve), _P, _P, _P, _I, _P, _P, _I, C.c_float, C.c_uint64, _P,
+                                      C.c_size_t, _P, _P]),
     "oea_nce_workspace_bytes": (C.c_size_t, [_I, _I, _I, _I]),
     "oea_nce_score_fed": (C.c_int, [C.POINTER(Nce), _P, _P, _I, _P, _P, _I, C.c_float, _P, C.c_size_t, _P, _P]),
     "oea_pairs_draw": (C.c_int, [_P, _I, _I, C.c_uint64, _I, _I, _P, _P, _P]),

@@ -28,7 +28,7 @@ class ProjE(BasicModel):
                          (a.ent_l2_norm is True and a.rel_l2_norm is True, "ent_l2_norm and rel_l2_norm"),
                          (a.dnn_neg_nums > 1, "dnn_neg_nums > 1")):
             if not ok:
-                raise ValueError("ProjE needs %s" % what)
+                raise ValueError("%s needs %s" % (type(self).__name__, what))
         if a.dnn_neg_nums > self.kgs.entities_num:
             raise ValueError("dnn_neg_nums = %d exceeds the %d entities: the sampler's range is too small"
                              % (a.dnn_neg_nums, self.kgs.entities_num))
@@ -38,16 +38,21 @@ class ProjE(BasicModel):
 
     def _define_variables(self):
         super()._define_variables()                      # ent_embeds, rel_embeds: xavier, l2-normalised, Adam slots
-        n_ent, d = self.kgs.entities_num, self.args.dim
-        self.entity_w = initializers.init_embeddings([n_ent, d], 'entity_w', 'xavier', False, optimizer='Adam')
-        # entity_b: xavier on the 1-D shape [E] (σ = sqrt(1.3/E)), stored as an [E, 1] table
-        self.entity_b = initializers._make(initializers.init_values([n_ent], 'xavier').reshape(n_ent, 1), False, 'Adam')
+        self._define_head_variables()
         # mlp/mlp_w and mlp/mlp_bias: get_variable's default glorot-uniform on [d] (limit sqrt(3/d)); both batch-norm
         # betas start at 0.  One [4, d] table: rows mlp_w, mlp_bias, input beta, output beta
+        d = self.args.dim
         lim = math.sqrt(3.0 / d)
         glorot = lambda: torch.rand(d, generator=initializers._GEN, dtype=torch.float32) * (2 * lim) - lim
         params = torch.stack([glorot(), glorot(), torch.zeros(d), torch.zeros(d)])
         self.proje_params = initializers._make(params, False, 'Adam')
+
+    def _define_head_variables(self):
+        """entity_w and entity_b, the NCE head's variables (proje.py:42-44)."""
+        n_ent, d = self.kgs.entities_num, self.args.dim
+        self.entity_w = initializers.init_embeddings([n_ent, d], 'entity_w', 'xavier', False, optimizer='Adam')
+        # entity_b: xavier on the 1-D shape [E] (σ = sqrt(1.3/E)), stored as an [E, 1] table
+        self.entity_b = initializers._make(initializers.init_values([n_ent], 'xavier').reshape(n_ent, 1), False, 'Adam')
 
     def _define_embed_graph(self):
         self.triple_trainer = eng.ProjETrainer((self.ent_embeds, self.rel_embeds, self.entity_w, self.entity_b,

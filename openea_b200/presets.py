@@ -96,6 +96,15 @@ def proje(scale="15K"):
                  start_valid=100 if small else 300, eval_metric="inner", eval_norm=True)
 
 
+def conve(scale="15K"):
+    """run/args/conve_args_15K.json and conve_args_100K.json: ProjE's settings plus the tower's."""
+    a = proje(scale)
+    a.embedding_module = "ConvE"
+    a.output_keep_prob = 0.7
+    a.filter_num = 32
+    return a
+
+
 def simple(scale="15K"):
     return _args(embedding_module="SimplE", alignment_module="sharing", dim=100, init="xavier", ent_l2_norm=True,
                  rel_l2_norm=True, learning_rate=0.01, optimizer="Adagrad", batch_size=5000 if scale == "15K" else 20000,
