@@ -30,7 +30,8 @@
 //   4. k_nce_dx             dX = G·W_S, split over the sampled set so that a batch of 500 still fills the machine
 //   5. k_nce_dw             dW_S = Gᵀ·X, split over the batch, pushed with red.global.add.v4.f32 (a sampled row may also
 //                           be a label row)
-//   6. k_proje_true         one warp per positive: the true logit, its loss, g = σ(t) − 1 into dX, entity_w and entity_b
+//   6. k_nce_true           one warp per positive, scale 1 over the raw entity_w: the true logit, its loss, g = σ(t) − 1
+//                           into dX, entity_w and entity_b
 //   7. k_proje_columns_bwd  one CTA per column: back through the three BNs and the combination; the gradients of mlp_w,
 //                           mlp_bias and both betas are this CTA's column sums
 //   8. k_proje_push         one warp per positive: dx_h, dx_r through the tables' normalisation into ent.grad, rel.grad
@@ -51,11 +52,11 @@
 // oea_conve_score_fed (models/neural/conve.py:42-79): two memsets and thirteen kernels, ProjE's head among them unchanged:
 //   1. k_conve_conv_fwd     one CTA per positive: the stacked image, its batch norm and dropout (kept in img), the 3×3
 //                           convolution, the per-filter batch norm, ReLU and dropout → A [n, 2Fd]
-//   2. k_conve_fc_fwd       Z = A·W on the head's register tile, split over the 2Fd inputs; k_conve_fc_out: bias, ReLU and
-//                           the output batch norm → X
-//   3. the head: k_nce_logq, k_nce_logits / k_nce_dx / k_nce_dw <GatheredW>, k_proje_true
-//   4. k_conve_fc_out_bwd   dX → dz; k_conve_fc_dw: dW = Aᵀ·dz; k_conve_fc_dx: dA = dz·Wᵀ through the ReLU and dropout,
-//                           written over A
+//   2. k_nce_dx<StagedW>    Z = A·W: the head's dX kernel with G := A, S := 2Fd and W_S := fc_w, split over the 2Fd
+//                           inputs; k_conve_fc_out: bias, ReLU and the output batch norm → X
+//   3. the head: k_nce_logq, k_nce_logits / k_nce_dx / k_nce_dw <GatheredW>, k_nce_true
+//   4. k_conve_fc_out_bwd   dX → dz; k_nce_dw<StagedW>: dW = Aᵀ·dz (the head's dW kernel, G := A, X := dz);
+//                           k_conve_fc_dx: dA = dz·Wᵀ through the ReLU and dropout, written over A
 //   5. k_conve_conv_dw      the convolution's and its batch norm's gradients per filter; k_conve_conv_dx: one CTA per
 //                           positive back to the image, through its dropout and batch norm, and into ent.grad, rel.grad
 //
@@ -72,31 +73,39 @@ constexpr int kTile = 128;                        // GEMM tile: 128 × 128 outpu
 constexpr int kTk = 16;                           // reduction slice staged per iteration
 constexpr int kTld = kTile + 4;                   // shared row stride of a staged slice
 
+// a row width in floats rounded up to whole float4s: table pitches, and the row strides of G and ConvE's A
+constexpr int round4(int v) { return (v + 3) / 4 * 4; }
+
+// a workspace cut into sections in the order they are taken, each 256-B aligned; `at` ends as the total
+struct WsCarver {
+    size_t at = 0;
+    size_t take(size_t bytes) { const size_t o = at; at += (bytes + 255) & ~(size_t)255; return o; }
+};
+
 struct ProjeWs {
     size_t first, xh, xr, z, x, dx, dxh, dxr, stats, lq, g, total;
     int ldg;                                      // row stride of G: S rounded up to 4
 };
 
-// workspace sections, each 256-B aligned: the sampler's first-draw index per class, then per positive six rows of
-// `pitch` floats, eight rows of column statistics, log q of every sampled class, and G [n_pos, ldg]
+// workspace sections: the sampler's first-draw index per class, then per positive six rows of `pitch` floats, eight
+// rows of column statistics, log q of every sampled class, and G [n_pos, ldg]
 static ProjeWs proje_layout(int n_pos, int num_sampled, int pitch, int n_classes) {
     ProjeWs w;
-    size_t at = 0;
-    auto take = [&](size_t bytes) { const size_t o = at; at += (bytes + 255) & ~(size_t)255; return o; };
+    WsCarver c;
     const size_t row = 4 * (size_t)n_pos * pitch;
-    w.ldg = (num_sampled + 3) / 4 * 4;
-    w.first = take(4 * (size_t)n_classes);
-    w.xh = take(row);
-    w.xr = take(row);
-    w.z = take(row);
-    w.x = take(row);
-    w.dx = take(row);
-    w.dxh = take(row);
-    w.dxr = take(row);
-    w.stats = take(4 * 8 * (size_t)pitch);
-    w.lq = take(4 * (size_t)num_sampled);
-    w.g = take(4 * (size_t)n_pos * w.ldg);
-    w.total = at;
+    w.ldg = round4(num_sampled);
+    w.first = c.take(4 * (size_t)n_classes);
+    w.xh = c.take(row);
+    w.xr = c.take(row);
+    w.z = c.take(row);
+    w.x = c.take(row);
+    w.dx = c.take(row);
+    w.dxh = c.take(row);
+    w.dxr = c.take(row);
+    w.stats = c.take(4 * 8 * (size_t)pitch);
+    w.lq = c.take(4 * (size_t)num_sampled);
+    w.g = c.take(4 * (size_t)n_pos * w.ldg);
+    w.total = c.at;
     return w;
 }
 
@@ -181,6 +190,8 @@ k_nce_logq(const int32_t* __restrict__ sampled, const int32_t* __restrict__ num_
 
 __device__ __forceinline__ float sigmoid_acc(float x) { return 1.f / (1.f + expf(-x)); }
 
+// num_sampled and ldg are the columns of G and its row stride: the sampled set's size S and round4(S) in the head, and
+// 2Fd and A's row stride when ConvE's dense layer runs on k_nce_dx / k_nce_dw with G := A
 struct ProjeDev {
     TableDev ent, rel, w, b, prm;
     int dim, pitch, n_classes, num_sampled, ldg;
@@ -200,7 +211,7 @@ struct GatheredW {
     __device__ __forceinline__ float scaled(float v) const { return v; }
 };
 // oea_nce_score_fed: ŵ_S staged contiguously by k_nce_stage, dŴ_S accumulated in the workspace (k_nce_w_push takes it
-// through the normalisation), loss and every gradient times `scale`
+// through the normalisation), loss and every gradient times `scale`.  ConvE's dense layer: fc_w and its gradient.
 struct StagedW {
     const float* w;
     float* dw;
@@ -547,61 +558,28 @@ k_nce_dw(ProjeDev T, int n, const float* __restrict__ G, const float* __restrict
     }
 }
 
-// the true class of every positive: logit, loss, and its whole backward (dX row, entity_w and entity_b rows)
-__global__ void __launch_bounds__(kThreads)
-k_proje_true(ProjeDev T, const int32_t* __restrict__ pt, int n, const float* __restrict__ x,
-             const int32_t* __restrict__ num_tries, float* __restrict__ dx, double* __restrict__ loss_out) {
-    __shared__ double s_loss[kWarpsPerBlock];
-    const int lane = threadIdx.x & 31;
-    const int tries = *num_tries;
-    float lsum = 0.f;
-    for (int b0 = (blockIdx.x * blockDim.x) >> 5; b0 < n; b0 += (gridDim.x * blockDim.x) >> 5) {   // warp-uniform
-        const int b = b0 + (threadIdx.x >> 5);
-        if (b >= n) continue;
-        const int c = __ldg(pt + b);
-        const Row<1> xb = load_row<1>(x, b, T.pitch, lane), wc = load_row<1>(T.w.w, c, T.pitch, lane);
-        const float logit = warp_sum(dotr(xb, wc)) + T.b.w[(size_t)c * T.b.pitch] -
-                            log_expected_count(c, T.n_classes, T.num_sampled, tries);
-        const float g = -sigmoid_acc(-logit);             // σ(t) − 1
-        if (lane == 0) {
-            lsum += softplus(-logit);
-            atomicAdd(T.b.g + (size_t)c * T.b.pitch, g);
-            T.b.touched[c] = 1;
-            T.w.touched[c] = 1;
-        }
-        if (4 * lane < T.pitch) {
-            float4* d = reinterpret_cast<float4*>(dx + (size_t)b * T.pitch + 4 * lane);
-            *d = fma4(wc.v[0], g, *d);
-        }
-        red_row<1>(T.w.g, c, T.pitch, lane, r_scale(xb, g));
-    }
-    LossAcc lacc{s_loss};
-    lacc.flush(warp_sum(lsum), loss_out);
-}
-
 // ---- the general sampled-NCE step (oea_nce_score_fed) ---------------------------------------------------------------
 struct NceWs {
     size_t first, x, dx, w, dw, winv, wss, lq, g, total;
     int ldg;
 };
 
-// workspace sections, each 256-B aligned: the sampler's first-draw index per class, x̂ and dX̂ [n, pitch], ŵ_S and dŴ_S
-// [S, pitch], 1/‖w_s‖ and Σw_s² [S], log q [S], G [n, ldg]
+// workspace sections: the sampler's first-draw index per class, x̂ and dX̂ [n, pitch], ŵ_S and dŴ_S [S, pitch],
+// 1/‖w_s‖ and Σw_s² [S], log q [S], G [n, ldg]
 static NceWs nce_layout(int n, int num_sampled, int pitch, int n_classes) {
     NceWs w;
-    size_t at = 0;
-    auto take = [&](size_t bytes) { const size_t o = at; at += (bytes + 255) & ~(size_t)255; return o; };
-    w.ldg = (num_sampled + 3) / 4 * 4;
-    w.first = take(4 * (size_t)n_classes);
-    w.x = take(4 * (size_t)n * pitch);
-    w.dx = take(4 * (size_t)n * pitch);
-    w.w = take(4 * (size_t)num_sampled * pitch);
-    w.dw = take(4 * (size_t)num_sampled * pitch);
-    w.winv = take(4 * (size_t)num_sampled);
-    w.wss = take(4 * (size_t)num_sampled);
-    w.lq = take(4 * (size_t)num_sampled);
-    w.g = take(4 * (size_t)n * w.ldg);
-    w.total = at;
+    WsCarver c;
+    w.ldg = round4(num_sampled);
+    w.first = c.take(4 * (size_t)n_classes);
+    w.x = c.take(4 * (size_t)n * pitch);
+    w.dx = c.take(4 * (size_t)n * pitch);
+    w.w = c.take(4 * (size_t)num_sampled * pitch);
+    w.dw = c.take(4 * (size_t)num_sampled * pitch);
+    w.winv = c.take(4 * (size_t)num_sampled);
+    w.wss = c.take(4 * (size_t)num_sampled);
+    w.lq = c.take(4 * (size_t)num_sampled);
+    w.g = c.take(4 * (size_t)n * w.ldg);
+    w.total = c.at;
     return w;
 }
 
@@ -629,7 +607,8 @@ k_nce_gather(ProjeDev T, const int32_t* __restrict__ ids, int n, float* __restri
 }
 
 // the true class of every row: ŵ_label normalised here, the logit, the loss, dX, and the label row's part of its
-// gradient through the normalisation
+// gradient through the normalisation.  ProjE and ConvE run it at scale 1 over their raw entity_w, where lookup and push
+// scale by exactly 1.
 __global__ void __launch_bounds__(kThreads)
 k_nce_true(ProjeDev T, const int32_t* __restrict__ labels, int n, const float* __restrict__ x,
            const int32_t* __restrict__ num_tries, float scale, float* __restrict__ dx, double* __restrict__ loss_out) {
@@ -698,10 +677,14 @@ k_pairs_draw(const int32_t* __restrict__ pairs, uint32_t n, int batch, uint64_t 
     }
 }
 
-// grids of the head's kernels for a batch of n and S sampled classes
+// grids of the head's kernels for a batch of n and S sampled classes.  ConvE's dense layer takes its own for (n, 2Fd,
+// lda): its forward and dW run on k_nce_dx and k_nce_dw, and its dA kernel tiles [n, lda] as the logits tile [n, ldg].
 struct HeadGrids {
     int rows, lg, dx, dw, split_s, split_b;
 };
+
+// `len` cut into about `parts` pieces, each a multiple of kTk
+static int split_of(int len, int parts) { const int s = (len + parts - 1) / parts; return (s + kTk - 1) / kTk * kTk; }
 
 static HeadGrids head_grids(int n, int S, int ldg) {
     HeadGrids h;
@@ -713,9 +696,8 @@ static HeadGrids head_grids(int n, int S, int ldg) {
     h.rows = grid_for(n);
     h.lg = mt_b * ((ldg + kTile - 1) / kTile);
     // split each reduction so that about two CTAs per SM run: a batch of 500 is only four row tiles, and S = 4096
-    // only 32 column tiles.  A split is a multiple of kTk.
+    // only 32 column tiles
     const int want = 2 * sm_count_cached();
-    auto split_of = [](int len, int parts) { const int s = (len + parts - 1) / parts; return (s + kTk - 1) / kTk * kTk; };
     h.split_s = split_of(S, (want + mt_b - 1) / mt_b);
     h.split_b = split_of(n, (want + mt_s - 1) / mt_s);
     h.dx = mt_b * ((S + h.split_s - 1) / h.split_s);
@@ -794,37 +776,6 @@ k_conve_conv_fwd(ProjeDev T, ConveDev C, const int32_t* __restrict__ ph, const i
     }
 }
 
-// Z[b][:] += Σ_{k in split} A[b][k]·W[k][:] over tile t = (batch tile, split of the lda inputs); Z was zeroed
-__global__ void __launch_bounds__(kThreads)
-k_conve_fc_fwd(ProjeDev T, ConveDev C, int n, const float* __restrict__ A, int split, float* __restrict__ z) {
-    __shared__ __align__(16) float As[kTk * kTld];
-    __shared__ __align__(16) float Bs[kTk * kTld];
-    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-    const int mt = (n + kTile - 1) / kTile, st = (C.lda + split - 1) / split;
-    for (int t = blockIdx.x; t < mt * st; t += gridDim.x) {
-        const int m0 = (t % mt) * kTile, k0s = (t / mt) * split, k1s = min(C.lda, k0s + split), kw = min(k1s, C.K);
-        float acc[8][8];
-        zero_acc(acc);
-        for (int k0 = k0s; k0 < k1s; k0 += kTk) {
-            __syncthreads();
-            stage_rows_t(As, [&](int i) { return m0 + i < n ? A + (size_t)(m0 + i) * C.lda : nullptr; }, k0, k1s);
-            stage_rows_n(Bs, [&](int k) { return k0 + k < kw ? C.fc_w.w + (size_t)(k0 + k) * T.pitch : nullptr; }, T.pitch);
-            __syncthreads();
-            tile_mma(acc, As, Bs, ty, tx);
-        }
-#pragma unroll
-        for (int a = 0; a < 8; ++a) {
-            const int m = m0 + ty + 16 * a;
-            if (m >= n) continue;
-#pragma unroll
-            for (int b = 0; b < 8; ++b) {
-                const int c = tx + 16 * b;
-                if (c < T.dim) atomicAdd(z + (size_t)m * T.pitch + c, acc[a][b]);
-            }
-        }
-    }
-}
-
 // the dense layer's bias and ReLU and the output BN: z += bias (kept for the backward), X = γ₃·relu(z)/√(1+ε) + β₃
 __global__ void __launch_bounds__(kThreads)
 k_conve_fc_out(ProjeDev T, ConveDev C, int n, float* __restrict__ z, float* __restrict__ x) {
@@ -867,43 +818,6 @@ k_conve_fc_out_bwd(ProjeDev T, ConveDev C, int n, const float* __restrict__ z, f
     for (int r = gt; r < C.F; r += gs) C.conv.touched[r] = 1;
     if (gt < 2) C.bn_in.touched[gt] = 1;
     if (gt < 3) C.fc_out.touched[gt] = 1;
-}
-
-// dW[k][:] += Σ_{b in split} A[b][k]·dz[b][:] over tile t = (input tile, split of the batch)
-__global__ void __launch_bounds__(kThreads)
-k_conve_fc_dw(ProjeDev T, ConveDev C, int n, const float* __restrict__ A, const float* __restrict__ dz, int split) {
-    __shared__ __align__(16) float As[kTk * kTld];
-    __shared__ __align__(16) float Bs[kTk * kTld];
-    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-    const int mt = (C.K + kTile - 1) / kTile, bt = (n + split - 1) / split;
-    for (int t = blockIdx.x; t < mt * bt; t += gridDim.x) {
-        const int m0 = (t % mt) * kTile, b0 = (t / mt) * split, b1 = min(n, b0 + split);
-        float acc[8][8];
-        zero_acc(acc);
-        for (int k0 = b0; k0 < b1; k0 += kTk) {
-            __syncthreads();
-            // A's rows run along k, so the slice is staged without a transpose
-            stage_rows_n(As, [&](int k) { return k0 + k < b1 ? A + (size_t)(k0 + k) * C.lda + m0 : nullptr; },
-                         min(kTile, C.lda - m0));
-            stage_rows_n(Bs, [&](int k) { return k0 + k < b1 ? dz + (size_t)(k0 + k) * T.pitch : nullptr; }, T.pitch);
-            __syncthreads();
-            tile_mma(acc, As, Bs, ty, tx);
-        }
-        __syncthreads();
-        float* Cs = As;                                   // 16 rows at a time, as k_nce_dw
-#pragma unroll
-        for (int a = 0; a < 8; ++a) {
-#pragma unroll
-            for (int b = 0; b < 8; ++b) Cs[ty * kTld + tx + 16 * b] = acc[a][b];
-            __syncthreads();
-            for (int e = threadIdx.x; e < 16 * (kTile / 4); e += blockDim.x) {
-                const int r = e >> 5, c = 4 * (e & 31), k = m0 + r + 16 * a;
-                if (k < C.K && c < T.pitch)
-                    red_add4(C.fc_w.g + (size_t)k * T.pitch + c, *reinterpret_cast<const float4*>(Cs + r * kTld + c));
-            }
-            __syncthreads();
-        }
-    }
 }
 
 // dA = dz·Wᵀ, taken back through the conv ReLU and dropout in the epilogue and written over A: the ReLU was active and
@@ -1069,25 +983,41 @@ struct ConveWs {
     int ldg, lda;
 };
 
-// workspace sections, each 256-B aligned: the sampler's first-draw index per class, the dropped image [n, 2d], the dense
-// layer's input A [n, lda] (its gradient dp overwrites it in the backward), z, X and dX [n, pitch], log q [S], G [n, ldg]
+// workspace sections: the sampler's first-draw index per class, the dropped image [n, 2d], the dense layer's input
+// A [n, lda] (its gradient dp overwrites it in the backward), z, X and dX [n, pitch], log q [S], G [n, ldg]
 static ConveWs conve_layout(int n, int num_sampled, int dim, int pitch, int filters, int n_classes) {
     ConveWs w;
-    size_t at = 0;
-    auto take = [&](size_t bytes) { const size_t o = at; at += (bytes + 255) & ~(size_t)255; return o; };
+    WsCarver c;
     const size_t row = 4 * (size_t)n * pitch;
-    w.ldg = (num_sampled + 3) / 4 * 4;
-    w.lda = (2 * filters * dim + 3) / 4 * 4;
-    w.first = take(4 * (size_t)n_classes);
-    w.img = take(4 * (size_t)n * 2 * dim);
-    w.a = take(4 * (size_t)n * w.lda);
-    w.z = take(row);
-    w.x = take(row);
-    w.dx = take(row);
-    w.lq = take(4 * (size_t)num_sampled);
-    w.g = take(4 * (size_t)n * w.ldg);
-    w.total = at;
+    w.ldg = round4(num_sampled);
+    w.lda = round4(2 * filters * dim);
+    w.first = c.take(4 * (size_t)n_classes);
+    w.img = c.take(4 * (size_t)n * 2 * dim);
+    w.a = c.take(4 * (size_t)n * w.lda);
+    w.z = c.take(row);
+    w.x = c.take(row);
+    w.dx = c.take(row);
+    w.lq = c.take(4 * (size_t)num_sampled);
+    w.g = c.take(4 * (size_t)n * w.ldg);
+    w.total = c.at;
     return w;
+}
+
+// The argument checks all three sampled-NCE steps make once their tables have passed their own: cls_b is [C, 1] for
+// the C rows of cls_w, 1 ≤ num_sampled ≤ C, n ≥ 0, the sampled set, num_tries and loss_out are given, and so are the
+// batch's id arrays when n > 0 (`ids_given`); last the workspace, against the size `layout()` computes from the checked
+// shapes.  OEA_OK or the first error; the caller returns early on either, and when n == 0.
+template <class Layout>
+static int check_head(const oea_table* w, const oea_table* b, int num_sampled, int n, const int32_t* sampled,
+                      const int32_t* num_tries, const double* loss_out, bool ids_given, const void* workspace,
+                      size_t workspace_bytes, Layout layout) {
+    if (b->rows != w->rows || b->dim != 1) return OEA_ERR_SHAPE;
+    if (num_sampled < 1 || num_sampled > w->rows) return OEA_ERR_RANGE;
+    if (n < 0) return OEA_ERR_SHAPE;
+    if (sampled == nullptr || num_tries == nullptr || loss_out == nullptr) return OEA_ERR_NULL;
+    if (n > 0 && !ids_given) return OEA_ERR_NULL;
+    if (workspace == nullptr || workspace_bytes < layout() || !aligned16(workspace)) return OEA_ERR_WORKSPACE;
+    return OEA_OK;
 }
 
 }  // namespace oea
@@ -1096,7 +1026,7 @@ using namespace oea;
 
 extern "C" size_t oea_proje_workspace_bytes(int32_t n_pos, int32_t num_sampled, int32_t dim, int32_t n_classes) {
     if (n_pos < 0 || num_sampled < 1 || dim <= 0 || n_classes <= 0) return 0;
-    return proje_layout(n_pos, num_sampled, (dim + 3) / 4 * 4, n_classes).total;
+    return proje_layout(n_pos, num_sampled, round4(dim), n_classes).total;
 }
 
 extern "C" int oea_logu_sample_unique(int32_t range_max, int32_t num_sampled, uint64_t seed, int32_t* sampled,
@@ -1124,14 +1054,12 @@ extern "C" int oea_proje_score_fed(const oea_proje* model, const int32_t* pos_h,
     if (rel->dim != ent->dim || w->dim != ent->dim || rel->pitch != ent->pitch || w->pitch != ent->pitch ||
         prm->pitch != ent->pitch || ent->pitch > kProjeMaxPitch)
         return OEA_ERR_DIM;
-    if (b->rows != w->rows || b->dim != 1 || prm->rows != 4 || prm->dim != ent->dim) return OEA_ERR_SHAPE;
-    if (num_sampled < 1 || num_sampled > w->rows) return OEA_ERR_RANGE;
-    if (n_pos < 0) return OEA_ERR_SHAPE;
-    if (sampled == nullptr || num_tries == nullptr || loss_out == nullptr) return OEA_ERR_NULL;
-    if (n_pos > 0 && (!pos_h || !pos_r || !pos_t)) return OEA_ERR_NULL;
-    const ProjeWs L = proje_layout(n_pos, num_sampled, ent->pitch, w->rows);
-    if (workspace == nullptr || workspace_bytes < L.total || !aligned16(workspace)) return OEA_ERR_WORKSPACE;
-    if (n_pos == 0) return OEA_OK;
+    if (prm->rows != 4 || prm->dim != ent->dim) return OEA_ERR_SHAPE;
+    ProjeWs L{};
+    const int rc = check_head(w, b, num_sampled, n_pos, sampled, num_tries, loss_out, pos_h && pos_r && pos_t,
+                              workspace, workspace_bytes,
+                              [&] { return (L = proje_layout(n_pos, num_sampled, ent->pitch, w->rows)).total; });
+    if (rc != OEA_OK || n_pos == 0) return rc;
 
     char* ws = static_cast<char*>(workspace);
     float* xh = reinterpret_cast<float*>(ws + L.xh);
@@ -1164,7 +1092,7 @@ extern "C" int oea_proje_score_fed(const oea_proje* model, const int32_t* pos_h,
     OEA_LAUNCH(k_nce_logits<GatheredW>, H.lg, kThreads, 0, st, T, n, x, sampled, lq, G, loss_out, GatheredW{});
     OEA_LAUNCH(k_nce_dx<GatheredW>, H.dx, kThreads, 0, st, T, n, G, sampled, H.split_s, dx, GatheredW{});
     OEA_LAUNCH(k_nce_dw<GatheredW>, H.dw, kThreads, 0, st, T, n, G, x, sampled, H.split_b, GatheredW{});
-    OEA_LAUNCH(k_proje_true, rows_grid, kThreads, 0, st, T, pos_t, n, x, num_tries, dx, loss_out);
+    OEA_LAUNCH(k_nce_true, rows_grid, kThreads, 0, st, T, pos_t, n, x, num_tries, 1.f, dx, loss_out);
     OEA_LAUNCH(k_proje_columns_bwd, col_grid, kThreads, 0, st, T, n, xh, xr, z, dx, stats, dxh, dxr);
     OEA_LAUNCH(k_proje_push, rows_grid, kThreads, 0, st, T, pos_h, pos_r, n, dxh, dxr);
     OEA_LAUNCH_CHECK();
@@ -1173,7 +1101,7 @@ extern "C" int oea_proje_score_fed(const oea_proje* model, const int32_t* pos_h,
 
 extern "C" size_t oea_nce_workspace_bytes(int32_t n, int32_t num_sampled, int32_t dim, int32_t n_classes) {
     if (n < 0 || num_sampled < 1 || dim <= 0 || n_classes <= 0) return 0;
-    return nce_layout(n, num_sampled, (dim + 3) / 4 * 4, n_classes).total;
+    return nce_layout(n, num_sampled, round4(dim), n_classes).total;
 }
 
 extern "C" int oea_nce_score_fed(const oea_nce* model, const int32_t* inputs, const int32_t* labels, int32_t n,
@@ -1187,14 +1115,11 @@ extern "C" int oea_nce_score_fed(const oea_nce* model, const int32_t* inputs, co
     }
     const oea_table *in = model->in, *w = model->cls_w, *b = model->cls_b;
     if (w->dim != in->dim || w->pitch != in->pitch || in->pitch > kProjeMaxPitch) return OEA_ERR_DIM;
-    if (b->rows != w->rows || b->dim != 1) return OEA_ERR_SHAPE;
-    if (num_sampled < 1 || num_sampled > w->rows) return OEA_ERR_RANGE;
-    if (n < 0) return OEA_ERR_SHAPE;
-    if (sampled == nullptr || num_tries == nullptr || loss_out == nullptr) return OEA_ERR_NULL;
-    if (n > 0 && (!inputs || !labels)) return OEA_ERR_NULL;
-    const NceWs L = nce_layout(n, num_sampled, in->pitch, w->rows);
-    if (workspace == nullptr || workspace_bytes < L.total || !aligned16(workspace)) return OEA_ERR_WORKSPACE;
-    if (n == 0) return OEA_OK;
+    NceWs L{};
+    const int rc = check_head(w, b, num_sampled, n, sampled, num_tries, loss_out, inputs && labels,
+                              workspace, workspace_bytes,
+                              [&] { return (L = nce_layout(n, num_sampled, in->pitch, w->rows)).total; });
+    if (rc != OEA_OK || n == 0) return rc;
 
     char* ws = static_cast<char*>(workspace);
     float* x = reinterpret_cast<float*>(ws + L.x);
@@ -1246,7 +1171,7 @@ extern "C" int oea_pairs_draw(const int32_t* pairs, int32_t n_pairs, int32_t bat
 extern "C" size_t oea_conve_workspace_bytes(int32_t n_pos, int32_t num_sampled, int32_t dim, int32_t filters,
                                             int32_t n_classes) {
     if (n_pos < 0 || num_sampled < 1 || dim <= 0 || filters < 1 || n_classes <= 0) return 0;
-    return conve_layout(n_pos, num_sampled, dim, (dim + 3) / 4 * 4, filters, n_classes).total;
+    return conve_layout(n_pos, num_sampled, dim, round4(dim), filters, n_classes).total;
 }
 
 extern "C" int oea_conve_score_fed(const oea_conve* model, const int32_t* pos_h, const int32_t* pos_r,
@@ -1269,17 +1194,15 @@ extern "C" int oea_conve_score_fed(const oea_conve* model, const int32_t* pos_h,
     if (F < 1) return OEA_ERR_DIM;
     int fx, fy;
     conve_factor(d, &fx, &fy);
-    if (b->rows != w->rows || b->dim != 1 || conv->dim != kConvCols || bn_in->rows != 2 || bn_in->dim != fy ||
-        fc_w->rows != 2 * F * d || fc_w->dim != d || fc_out->rows != 3 || fc_out->dim != d)
+    if (conv->dim != kConvCols || bn_in->rows != 2 || bn_in->dim != fy || fc_w->rows != 2 * F * d || fc_w->dim != d ||
+        fc_out->rows != 3 || fc_out->dim != d)
         return OEA_ERR_SHAPE;
     if (!(keep_prob > 0.f && keep_prob <= 1.f)) return OEA_ERR_RANGE;
-    if (num_sampled < 1 || num_sampled > w->rows) return OEA_ERR_RANGE;
-    if (n_pos < 0) return OEA_ERR_SHAPE;
-    if (sampled == nullptr || num_tries == nullptr || loss_out == nullptr) return OEA_ERR_NULL;
-    if (n_pos > 0 && (!pos_h || !pos_r || !pos_t)) return OEA_ERR_NULL;
-    const ConveWs L = conve_layout(n_pos, num_sampled, d, P, F, w->rows);
-    if (workspace == nullptr || workspace_bytes < L.total || !aligned16(workspace)) return OEA_ERR_WORKSPACE;
-    if (n_pos == 0) return OEA_OK;
+    ConveWs L{};
+    const int rc = check_head(w, b, num_sampled, n_pos, sampled, num_tries, loss_out, pos_h && pos_r && pos_t,
+                              workspace, workspace_bytes,
+                              [&] { return (L = conve_layout(n_pos, num_sampled, d, P, F, w->rows)).total; });
+    if (rc != OEA_OK || n_pos == 0) return rc;
 
     char* ws = static_cast<char*>(workspace);
     float* img = reinterpret_cast<float*>(ws + L.img);
@@ -1296,25 +1219,21 @@ extern "C" int oea_conve_score_fed(const oea_conve* model, const int32_t* pos_h,
     ConveDev C;
     C.conv = table_dev(conv); C.bn_in = table_dev(bn_in); C.fc_w = table_dev(fc_w); C.fc_out = table_dev(fc_out);
     C.x = fx; C.y = fy; C.F = F; C.K = 2 * F * d; C.lda = L.lda; C.keep = keep_prob; C.seed = dropout_seed;
+    // the dense layer on the head's dX and dW kernels: G := A with 2Fd columns at row stride lda (its padding columns
+    // are zero, as G's are), W_S := fc_w as a contiguous block.  StagedW ignores the sampled ids.
+    ProjeDev Tfc = T;
+    Tfc.num_sampled = C.K; Tfc.ldg = L.lda;
+    const StagedW fc{C.fc_w.w, C.fc_w.g, 1.f};
     cudaStream_t st = (cudaStream_t)stream;
     const int n = n_pos, S = num_sampled;
-    const HeadGrids H = head_grids(n, S, L.ldg);
+    const HeadGrids H = head_grids(n, S, L.ldg), Hfc = head_grids(n, C.K, L.lda);
 #ifdef OEA_HOST_EMU
-    const int pos_grid = 2, fwd_grid = 2, dw_grid = 2, dx_grid = 2, conv_grid = 2, out_grid = 2, bwd_grid = 2;
-    const int split_k = 2 * kTk, split_b = 2 * kTk, split_conv = 7;
+    const int pos_grid = 2, conv_grid = 2, out_grid = 2, bwd_grid = 2, split_conv = 7;
 #else
-    // split the dense layer's reductions so that about two CTAs per SM run (a batch of 500 is four row tiles; d = 100
-    // is one column tile), and the per-filter sums of the conv backward over about two CTAs per SM as well
-    const int sms = sm_count_cached(), want = 2 * sms;
-    const int mt_b = (n + kTile - 1) / kTile, mt_k = (C.K + kTile - 1) / kTile;
-    auto split_of = [](int len, int parts) { const int s = (len + parts - 1) / parts; return (s + kTk - 1) / kTk * kTk; };
-    const int split_k = split_of(L.lda, (want + mt_b - 1) / mt_b);
-    const int split_b = split_of(n, (want + mt_k - 1) / mt_k);
-    const int conv_parts = (want + F - 1) / F, split_conv = (n + conv_parts - 1) / conv_parts;
+    // split the per-filter sums of the conv backward so that about two CTAs per SM run
+    const int sms = sm_count_cached();
+    const int conv_parts = (2 * sms + F - 1) / F, split_conv = (n + conv_parts - 1) / conv_parts;
     const int pos_grid = min(n, 8 * sms);
-    const int fwd_grid = mt_b * ((L.lda + split_k - 1) / split_k);
-    const int dw_grid = mt_k * ((n + split_b - 1) / split_b);
-    const int dx_grid = mt_b * ((L.lda + kTile - 1) / kTile);
     const int conv_grid = F * ((n + split_conv - 1) / split_conv);
     const int out_grid = min((int)(((size_t)n * P + kThreads - 1) / kThreads), 8 * sms);
     const int bwd_grid = min((n + 1) / 2, sms);           // two rows per block step; one flush of 3·d sums per block
@@ -1322,16 +1241,16 @@ extern "C" int oea_conve_score_fed(const oea_conve* model, const int32_t* pos_h,
     OEA_CUDA_TRY(cudaMemsetAsync(z, 0, 4 * (size_t)n * P, st));
     OEA_CUDA_TRY(cudaMemsetAsync(dx, 0, 4 * (size_t)n * P, st));
     OEA_LAUNCH(k_conve_conv_fwd, pos_grid, kThreads, 0, st, T, C, pos_h, pos_r, n, img, A);
-    OEA_LAUNCH(k_conve_fc_fwd, fwd_grid, kThreads, 0, st, T, C, n, A, split_k, z);
+    OEA_LAUNCH(k_nce_dx<StagedW>, Hfc.dx, kThreads, 0, st, Tfc, n, A, sampled, Hfc.split_s, z, fc);
     OEA_LAUNCH(k_conve_fc_out, out_grid, kThreads, 0, st, T, C, n, z, x);
     OEA_LAUNCH(k_nce_logq, H.rows, kThreads, 0, st, sampled, num_tries, T.n_classes, S, lq);
     OEA_LAUNCH(k_nce_logits<GatheredW>, H.lg, kThreads, 0, st, T, n, x, sampled, lq, G, loss_out, GatheredW{});
     OEA_LAUNCH(k_nce_dx<GatheredW>, H.dx, kThreads, 0, st, T, n, G, sampled, H.split_s, dx, GatheredW{});
     OEA_LAUNCH(k_nce_dw<GatheredW>, H.dw, kThreads, 0, st, T, n, G, x, sampled, H.split_b, GatheredW{});
-    OEA_LAUNCH(k_proje_true, H.rows, kThreads, 0, st, T, pos_t, n, x, num_tries, dx, loss_out);
+    OEA_LAUNCH(k_nce_true, H.rows, kThreads, 0, st, T, pos_t, n, x, num_tries, 1.f, dx, loss_out);
     OEA_LAUNCH(k_conve_fc_out_bwd, bwd_grid, kThreads, 0, st, T, C, n, z, dx);
-    OEA_LAUNCH(k_conve_fc_dw, dw_grid, kThreads, 0, st, T, C, n, A, dx, split_b);
-    OEA_LAUNCH(k_conve_fc_dx, dx_grid, kThreads, 0, st, T, C, n, dx, A);
+    OEA_LAUNCH(k_nce_dw<StagedW>, Hfc.dw, kThreads, 0, st, Tfc, n, A, dx, sampled, Hfc.split_b, fc);
+    OEA_LAUNCH(k_conve_fc_dx, Hfc.lg, kThreads, 0, st, T, C, n, dx, A);
     OEA_LAUNCH(k_conve_conv_dw, conv_grid, kThreads, 0, st, T, C, n, img, A, split_conv);
     OEA_LAUNCH(k_conve_conv_dx, pos_grid, kThreads, 0, st, T, C, pos_h, pos_r, n, A);
     OEA_LAUNCH_CHECK();

@@ -30,6 +30,13 @@ def pitch_for(dim):
     return (int(dim) + 3) // 4 * 4
 
 
+def _grown(buf, need, device):
+    """`buf` if it holds `need` bytes, else a new byte buffer of that size (at least 1 B) on `device`."""
+    if buf is None or buf.numel() < need:
+        buf = torch.empty(max(1, need), dtype=torch.uint8, device=device)
+    return buf
+
+
 class EmbeddingTable:
     """A TF-style embedding variable + optimiser slots on the device.
 
@@ -446,8 +453,7 @@ class ModelTrainer:
     def _workspace(self, n_pos, n_neg):
         """TransR's scratch (bucketed triple ids, chunk list, scores, projections) for a batch of this size."""
         need = self.lib.oea_transr_workspace_bytes(n_pos, n_neg, self.tables[0].dim, self.tables[1].rows)
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(max(1, need), dtype=torch.uint8, device=self.tables[0].device)
+        self._ws = _grown(self._ws, need, self.tables[0].device)
         return self._ws
 
     def _c_model(self):
@@ -523,64 +529,90 @@ class ModelTrainer:
         return v
 
 
-class ProjETrainer:
-    """ProjE's step (models/neural/proje.py:46-96): device batch producer (oea_triple_sample_batch, positives only) →
-    TF's unique log-uniform sampler on the device (oea_logu_sample_unique; one set of `num_sampled` classes per step,
-    seeded from the epoch seed and the step) → the projection layer and the NCE head (oea_proje_score_fed) → Adam on the
-    five tables.  tables = (ent, rel, cls_w, cls_b, params) EmbeddingTables: entity_w, entity_b as [E, 1], and the
-    [4, d] table of mlp_w, mlp_bias and the two batch-norm betas.  The workspace grows on demand."""
+class SampledNceTrainer:
+    """What every step on the sampled-NCE head shares: TF's unique log-uniform sampler on the device
+    (oea_logu_sample_unique; one set of `num_sampled` classes per step, seeded from the epoch seed and the step) into
+    `sampled` / `num_tries`, the loss accumulated on the device (`loss_dev`, read_loss), a workspace that grows on demand
+    and one optimiser step over every table.  `n_classes` is the rows of the class table."""
 
-    def __init__(self, tables, num_sampled, lr, sampler="fast"):
+    def __init__(self, tables, num_sampled, lr, n_classes):
         self.lib = L.load()
         self.tables = tuple(tables)
         self.num_sampled = int(num_sampled)
-        n_classes = self.tables[2].rows
-        if not 1 <= self.num_sampled <= n_classes:
+        self.n_classes = int(n_classes)
+        if not 1 <= self.num_sampled <= self.n_classes:
             raise ValueError("nce_loss samples %d distinct classes out of %d: the sampler's range is too small"
-                             % (self.num_sampled, n_classes))
+                             % (self.num_sampled, self.n_classes))
         self.lr = float(lr)
-        self.sampler = {"fast": 0, "independent": 1}[sampler]
         dev = self.tables[0].device
         self.loss_dev = torch.zeros(1, dtype=torch.float64, device=dev)
         self.sampled = torch.zeros(self.num_sampled, dtype=torch.int32, device=dev)
         self.num_tries = torch.zeros(1, dtype=torch.int32, device=dev)
-        self._idx = None
-        self._n_pos = C.c_int32(0)
         self._ws = None
 
-    def _workspace(self, n_pos):
-        need = self.lib.oea_proje_workspace_bytes(n_pos, self.num_sampled, self.tables[0].dim, self.tables[2].rows)
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(max(1, need), dtype=torch.uint8, device=self.tables[0].device)
+    def _workspace(self, n):
+        """The step's scratch for a batch of n (n = 0: the sampler's alone); _workspace_bytes(n) sizes it."""
+        self._ws = _grown(self._ws, self._workspace_bytes(n), self.tables[0].device)
         return self._ws
-
-    def _c_model(self):
-        return L.Proje(*[C.pointer(t.c_struct()) for t in self.tables])
 
     def sample(self, seed):
         """Draw the step's sampled set into self.sampled / self.num_tries (device; no host synchronisation)."""
         ws = self._workspace(0)
-        L.check(self.lib.oea_logu_sample_unique(self.tables[2].rows, self.num_sampled, int(seed) & (2**64 - 1),
+        L.check(self.lib.oea_logu_sample_unique(self.n_classes, self.num_sampled, int(seed) & (2**64 - 1),
                                                 _ptr(self.sampled), _ptr(self.num_tries), _ptr(ws), ws.numel(),
                                                 _stream_ptr()), "oea_logu_sample_unique")
 
-    def score_fed(self, pos, sampled=None, num_tries=None, loss_out=None):
-        """pos: int32 device tensor [3, n] (h | r | t rows); sampled / num_tries: int32 device tensors (default: the
-        last sample()).  Accumulates gradients into the five tables and adds the batch loss into loss_out."""
-        out = self.loss_dev if loss_out is None else loss_out
+    def _score(self, fn, model, ids, n, sampled, num_tries, loss_out, *step_args):
+        """fn(model, *ids, n, sampled, num_tries, S, *step_args, workspace, its bytes, loss_out, stream): sampled /
+        num_tries default to the last sample(), loss_out to loss_dev."""
         sampled = self.sampled if sampled is None else sampled
         num_tries = self.num_tries if num_tries is None else num_tries
-        n_pos = pos.shape[1]
-        ws = self._workspace(n_pos)
-        model = self._c_model()
-        np_ = lambda i: C.c_void_p(0 if n_pos == 0 else pos[i].data_ptr())
-        L.check(self.lib.oea_proje_score_fed(C.byref(model), np_(0), np_(1), np_(2), n_pos, _ptr(sampled),
-                                             _ptr(num_tries), sampled.numel(), _ptr(ws), ws.numel(), _ptr(out),
-                                             _stream_ptr()), "oea_proje_score_fed")
+        ws = self._workspace(n)
+        L.check(getattr(self.lib, fn)(C.byref(model), *ids, n, _ptr(sampled), _ptr(num_tries), sampled.numel(),
+                                      *step_args, _ptr(ws), ws.numel(),
+                                      _ptr(self.loss_dev if loss_out is None else loss_out), _stream_ptr()), fn)
 
     def apply(self):
         for tab in self.tables:
             tab.apply(self.lr)
+
+    @staticmethod
+    def step_seed(epoch_seed, step):
+        """The sampler's seed of one step: a function of (epoch seed, step) only, so that a resumed run draws the same."""
+        return (int(epoch_seed) * 0x9E3779B97F4A7C15 + int(step) + 1) & (2**64 - 1)
+
+    def read_loss(self, reset=True):
+        v = float(self.loss_dev.item())
+        if reset:
+            self.loss_dev.zero_()
+        return v
+
+
+def _pos_rows(pos):
+    """The h, r and t rows of a [3, n] int32 device batch as C pointers (NULL for an empty batch)."""
+    return [C.c_void_p(0 if pos.shape[1] == 0 else pos[i].data_ptr()) for i in range(3)]
+
+
+class ProjETrainer(SampledNceTrainer):
+    """ProjE's step (models/neural/proje.py:46-96): device batch producer (oea_triple_sample_batch, positives only) →
+    the sampler → the projection layer and the NCE head (oea_proje_score_fed) → Adam on the five tables.
+    tables = (ent, rel, cls_w, cls_b, params) EmbeddingTables: entity_w, entity_b as [E, 1], and the [4, d] table of
+    mlp_w, mlp_bias and the two batch-norm betas."""
+
+    def __init__(self, tables, num_sampled, lr, sampler="fast"):
+        super().__init__(tables, num_sampled, lr, tables[2].rows)
+        self.sampler = {"fast": 0, "independent": 1}[sampler]
+        self._idx = None
+        self._n_pos = C.c_int32(0)
+
+    def _workspace_bytes(self, n_pos):
+        return self.lib.oea_proje_workspace_bytes(n_pos, self.num_sampled, self.tables[0].dim, self.n_classes)
+
+    def score_fed(self, pos, sampled=None, num_tries=None, loss_out=None):
+        """pos: int32 device tensor [3, n] (h | r | t rows); sampled / num_tries: int32 device tensors (default: the
+        last sample()).  Accumulates gradients into the five tables and adds the batch loss into loss_out."""
+        self._score("oea_proje_score_fed", L.Proje(*[C.pointer(t.c_struct()) for t in self.tables]), _pos_rows(pos),
+                    pos.shape[1], sampled, num_tries, loss_out)
 
     def sample_batch(self, kg1, kg2, tset, batch_size, step, epoch_seed, max_try=10):
         """The device batch producer with no negatives: pos [3, n_pos] int32 device tensor."""
@@ -594,11 +626,6 @@ class ProjETrainer:
         n = int(self._n_pos.value)
         return self._idx[:3 * n].view(3, n)
 
-    @staticmethod
-    def step_seed(epoch_seed, step):
-        """The sampler's seed of one step: a function of (epoch seed, step) only, so that a resumed run draws the same."""
-        return (int(epoch_seed) * 0x9E3779B97F4A7C15 + int(step) + 1) & (2**64 - 1)
-
     def step_sampled(self, kg1, kg2, tset, batch_size, neg_per_pos, step, epoch_seed, max_try=10, **_):
         """One session.run([triple_loss, triple_optimizer]) of proje.py:87-90; neg_per_pos is ignored (positives only)."""
         pos = self.sample_batch(kg1, kg2, tset, batch_size, step, epoch_seed, max_try)
@@ -608,12 +635,6 @@ class ProjETrainer:
         self.score_fed(pos)
         self.apply()
         return pos.shape[1]
-
-    def read_loss(self, reset=True):
-        v = float(self.loss_dev.item())
-        if reset:
-            self.loss_dev.zero_()
-        return v
 
 
 class ConvETrainer(ProjETrainer):
@@ -629,27 +650,15 @@ class ConvETrainer(ProjETrainer):
             raise ValueError("output_keep_prob = %r is not in (0, 1]" % keep_prob)
         self.filters = self.tables[4].rows
 
-    def _workspace(self, n_pos):
-        need = self.lib.oea_conve_workspace_bytes(n_pos, self.num_sampled, self.tables[0].dim, self.filters,
-                                                  self.tables[2].rows)
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(max(1, need), dtype=torch.uint8, device=self.tables[0].device)
-        return self._ws
+    def _workspace_bytes(self, n_pos):
+        return self.lib.oea_conve_workspace_bytes(n_pos, self.num_sampled, self.tables[0].dim, self.filters,
+                                                  self.n_classes)
 
     def score_fed(self, pos, sampled=None, num_tries=None, dropout_seed=0, loss_out=None):
         """pos: int32 device tensor [3, n] (h | r | t rows); sampled / num_tries: int32 device tensors (default: the
         last sample()).  Accumulates gradients into the eight tables and adds the batch loss into loss_out."""
-        out = self.loss_dev if loss_out is None else loss_out
-        sampled = self.sampled if sampled is None else sampled
-        num_tries = self.num_tries if num_tries is None else num_tries
-        n_pos = pos.shape[1]
-        ws = self._workspace(n_pos)
-        model = L.Conve(*[C.pointer(t.c_struct()) for t in self.tables])
-        np_ = lambda i: C.c_void_p(0 if n_pos == 0 else pos[i].data_ptr())
-        L.check(self.lib.oea_conve_score_fed(C.byref(model), np_(0), np_(1), np_(2), n_pos, _ptr(sampled),
-                                             _ptr(num_tries), sampled.numel(), self.keep_prob,
-                                             int(dropout_seed) & (2**64 - 1), _ptr(ws), ws.numel(), _ptr(out),
-                                             _stream_ptr()), "oea_conve_score_fed")
+        self._score("oea_conve_score_fed", L.Conve(*[C.pointer(t.c_struct()) for t in self.tables]), _pos_rows(pos),
+                    pos.shape[1], sampled, num_tries, loss_out, self.keep_prob, int(dropout_seed) & (2**64 - 1))
 
     def step_sampled(self, kg1, kg2, tset, batch_size, neg_per_pos, step, epoch_seed, max_try=10, **_):
         """One session.run([triple_loss, triple_optimizer]) of conve.py:42-79; neg_per_pos is ignored (positives only)."""
@@ -663,35 +672,19 @@ class ConvETrainer(ProjETrainer):
         return pos.shape[1]
 
 
-class NceTrainer:
+class NceTrainer(SampledNceTrainer):
     """tf.nn.nce_loss applied to an embedding lookup, one reduce_mean step of approaches/attr2vec.py:113-124,145-161:
-    B distinct pairs drawn on the device (oea_pairs_draw, keyed by (seed, epoch, step)) → TF's unique log-uniform
-    sampler (oea_logu_sample_unique, seeded from the epoch seed and the step as ProjETrainer does) →
-    oea_nce_score_fed with loss_scale 1/B → Adagrad (or the tables' optimiser) on the three tables.
-    tables = (inputs, cls_w, cls_b) EmbeddingTables, cls_b as [C, 1].  Losses accumulate on the device (read_loss)."""
+    B distinct pairs drawn on the device (oea_pairs_draw, keyed by (seed, epoch, step)) → the sampler, seeded from the
+    seed, the epoch and the step → oea_nce_score_fed with loss_scale 1/B → Adagrad (or the tables' optimiser) on the
+    three tables.  tables = (inputs, cls_w, cls_b) EmbeddingTables, cls_b as [C, 1]."""
 
     def __init__(self, tables, num_sampled, lr):
-        self.lib = L.load()
-        self.tables = tuple(tables)
-        self.num_sampled = int(num_sampled)
-        n_classes = self.tables[1].rows
-        if not 1 <= self.num_sampled <= n_classes:
-            raise ValueError("nce_loss samples %d distinct classes out of %d: the sampler's range is too small"
-                             % (self.num_sampled, n_classes))
-        self.lr = float(lr)
-        dev = self.tables[0].device
-        self.loss_dev = torch.zeros(1, dtype=torch.float64, device=dev)
-        self.sampled = torch.zeros(self.num_sampled, dtype=torch.int32, device=dev)
-        self.num_tries = torch.zeros(1, dtype=torch.int32, device=dev)
+        super().__init__(tables, num_sampled, lr, tables[1].rows)
         self.pairs = None
         self._batch = None
-        self._ws = None
 
-    def _workspace(self, n):
-        need = self.lib.oea_nce_workspace_bytes(n, self.num_sampled, self.tables[0].dim, self.tables[1].rows)
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(max(1, need), dtype=torch.uint8, device=self.tables[0].device)
-        return self._ws
+    def _workspace_bytes(self, n):
+        return self.lib.oea_nce_workspace_bytes(n, self.num_sampled, self.tables[0].dim, self.n_classes)
 
     def set_pairs(self, pairs):
         """The training pairs the steps draw from: [n, 2] (input id, label id), copied to the device once."""
@@ -706,44 +699,21 @@ class NceTrainer:
                                         _stream_ptr()), "oea_pairs_draw")
         return self._batch[0, :batch], self._batch[1, :batch]
 
-    def sample(self, seed):
-        """Draw the step's sampled set into self.sampled / self.num_tries (device; no host synchronisation)."""
-        ws = self._workspace(0)
-        L.check(self.lib.oea_logu_sample_unique(self.tables[1].rows, self.num_sampled, int(seed) & (2**64 - 1),
-                                                _ptr(self.sampled), _ptr(self.num_tries), _ptr(ws), ws.numel(),
-                                                _stream_ptr()), "oea_logu_sample_unique")
-
     def score_fed(self, inputs, labels, sampled=None, num_tries=None, scale=None, loss_out=None):
         """inputs / labels: int32 device tensors [n]; sampled / num_tries: int32 device tensors (default: the last
         sample()); scale: default 1/n (reduce_mean).  Accumulates gradients into the three tables and adds the scaled
         batch loss into loss_out."""
-        out = self.loss_dev if loss_out is None else loss_out
-        sampled = self.sampled if sampled is None else sampled
-        num_tries = self.num_tries if num_tries is None else num_tries
         n = inputs.numel()
         scale = 1.0 / max(1, n) if scale is None else float(scale)
-        ws = self._workspace(n)
-        model = L.Nce(*[C.pointer(t.c_struct()) for t in self.tables])
-        L.check(self.lib.oea_nce_score_fed(C.byref(model), _ptr(inputs), _ptr(labels), n, _ptr(sampled),
-                                           _ptr(num_tries), sampled.numel(), scale, _ptr(ws), ws.numel(), _ptr(out),
-                                           _stream_ptr()), "oea_nce_score_fed")
-
-    def apply(self):
-        for tab in self.tables:
-            tab.apply(self.lr)
+        self._score("oea_nce_score_fed", L.Nce(*[C.pointer(t.c_struct()) for t in self.tables]),
+                    (_ptr(inputs), _ptr(labels)), n, sampled, num_tries, loss_out, scale)
 
     def step(self, batch, seed, epoch, step):
         """One session.run([loss, optimizer]) of attr2vec.py:156-158 on pairs drawn from set_pairs()."""
         inputs, labels = self.draw(batch, seed, epoch, step)
-        self.sample(ProjETrainer.step_seed(ProjETrainer.step_seed(seed, epoch), step))
+        self.sample(self.step_seed(self.step_seed(seed, epoch), step))
         self.score_fed(inputs, labels)
         self.apply()
-
-    def read_loss(self, reset=True):
-        v = float(self.loss_dev.item())
-        if reset:
-            self.loss_dev.zero_()
-        return v
 
 
 class FedHostPipeline:

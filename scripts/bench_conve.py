@@ -19,8 +19,9 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from openea_b200 import engine as eng  # noqa: E402
 from scripts.bench_proje import SHAPES, card  # noqa: E402
 
-HEAD = ("k_nce_logq", "k_nce_logits", "k_nce_dx", "k_nce_dw", "k_proje_true")
-FC = ("k_conve_fc_fwd", "k_conve_fc_dw", "k_conve_fc_dx")
+# the head's dX and dW kernels also run the dense layer's forward and dW: their template argument tells them apart
+HEAD = ("k_nce_logq", "k_nce_logits", "k_nce_dx<oea::GatheredW>", "k_nce_dw<oea::GatheredW>", "k_nce_true")
+FC = ("k_nce_dx<oea::StagedW>", "k_nce_dw<oea::StagedW>", "k_conve_fc_dx")
 TOWER = FC + ("k_conve_conv_fwd", "k_conve_fc_out", "k_conve_fc_out_bwd", "k_conve_conv_dw", "k_conve_conv_dx")
 
 

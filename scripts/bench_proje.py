@@ -20,7 +20,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from openea_b200 import engine as eng  # noqa: E402
 
 SHAPES = {"15K": (500, 30000, 1000), "100K": (5000, 200000, 1500)}     # (batch, entities, relations)
-HEAD = ("k_nce_logits", "k_nce_dx", "k_nce_dw", "k_proje_true")
+HEAD = ("k_nce_logits", "k_nce_dx", "k_nce_dw", "k_nce_true")
 PROJ = ("k_proje_gather", "k_proje_columns_fwd", "k_proje_columns_bwd", "k_proje_push")
 
 
